@@ -1,4 +1,4 @@
-# Build of libabpoa_b200.so (host C + sm_100a CUDA) and of the test-only oracle.
+# Build of libabpoa_b200.so (host C + sm_90a CUDA) and of the test-only oracle.
 #   make            -> abpoa_b200/lib/libabpoa_b200.so
 #   make oracle     -> oracle/libpoa_oracle.so (+ oracle/_ref/ when /root/reference exists)
 NVCC    ?= /usr/local/cuda/bin/nvcc
@@ -7,7 +7,7 @@ CSRC    := abpoa_b200/csrc
 OBJ     := build/obj
 LIBDIR  := abpoa_b200/lib
 LIB     := $(LIBDIR)/libabpoa_b200.so
-ARCH    := -gencode arch=compute_100a,code=sm_100a
+ARCH    := -gencode arch=compute_90a,code=sm_90a
 CFLAGS  := -O2 -g -Wall -Wextra -Wno-unused-parameter -fPIC -Iinclude -I$(CSRC) -std=gnu11 -pthread
 NVFLAGS := $(KPROF) $(ARCH) -O3 -lineinfo -std=c++17 -Xcompiler -fPIC,-Wall,-pthread -Iinclude -I$(CSRC)
 

@@ -1,7 +1,7 @@
-"""abpoa_b200 -- B200-native adaptive-banded partial-order alignment.
+"""abpoa_b200 -- H100-native adaptive-banded partial-order alignment.
 
 The product is the C-ABI shared library ``abpoa_b200/lib/libabpoa_b200.so`` (host C behind
-abPOA's ``abpoa.h`` interface + hand-written sm_100a CUDA kernels, built by
+abPOA's ``abpoa.h`` interface + hand-written sm_90a CUDA kernels, built by
 ``__graft_entry__.build()`` / ``make``).  This package is the thin Python host-side mirror of
 the reference's Python interface (pyabpoa) on top of that library.
 """

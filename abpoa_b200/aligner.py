@@ -1,7 +1,7 @@
 """Host-side mirror of the reference's Python interface (python/pyabpoa.pyx:9-371).
 
 ``msa_aligner`` / ``msa_result`` keep pyabpoa's names, arguments and result fields, but the
-calls go through the abpoa.h C ABI of a shared object -- by default the B200 library
+calls go through the abpoa.h C ABI of a shared object -- by default the GPU library
 (``libabpoa_b200.so``), whose alignments run in CUDA kernels.  Passing ``lib=`` lets the test
 suite run the very same driver over ``oracle/_ref/libabpoa_ref.so`` (the unmodified
 reference) to compare results; the product path never does that.
@@ -285,7 +285,7 @@ class msa_result:
 
 
 class msa_aligner:
-    """pyabpoa.msa_aligner (python/pyabpoa.pyx:93-371) over the B200 library: same constructor arguments, same
+    """pyabpoa.msa_aligner (python/pyabpoa.pyx:93-371) over the GPU library: same constructor arguments, same
     methods (msa, msa_align, msa_add, msa_output), same result fields.  One handle lives as long as the object,
     so msa_align / msa_add / msa_output build a graph incrementally exactly as the Cython class does."""
 

@@ -1,6 +1,6 @@
 """ctypes binding of include/abpoa_gpu.h -- the batched, multi-stream engine.
 
-``BatchEngine.run(cfg, groups)`` is what fills a B200: it advances many independent read groups
+``BatchEngine.run(cfg, groups)`` is what fills a GPU: it advances many independent read groups
 concurrently (one warp per alignment, worker threads fusing graph-CIGARs on the host while other
 chunks compute) and returns, per group, what ``abpoa_msa()`` would have left in ``ab->abc``.
 """

@@ -1,7 +1,7 @@
 """ctypes view of the abpoa.h C ABI (include/abpoa.h; reference include/abpoa.h:58-230).
 
 The Structure definitions bind ANY shared object that exports this ABI: the product
-(``abpoa_b200/lib/libabpoa_b200.so``: host C + sm_100a CUDA kernels) through ``product()``, and -- from the
+(``abpoa_b200/lib/libabpoa_b200.so``: host C + sm_90a CUDA kernels) through ``product()``, and -- from the
 test suite and the benchmark's reference arm only, which locate it themselves -- the unmodified reference
 built by ``oracle/Makefile``, through ``load_library(path)``; a parity test is literally "run the same calls
 through two libraries and compare".  Nothing in this package knows where the reference lives.
@@ -211,7 +211,7 @@ def load_library(path: os.PathLike | str) -> PoaLibrary:
 
 
 def product() -> PoaLibrary:
-    """The B200 library.  Raises if it has not been built - there is no fallback."""
+    """The GPU library.  Raises if it has not been built - there is no fallback."""
     override = os.environ.get("ABPOA_B200_LIB")          # experiments: another build of the same library
     return load_library(Path(override) if override else PRODUCT_LIB)
 

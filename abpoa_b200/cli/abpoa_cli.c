@@ -28,7 +28,7 @@ static const struct option long_opt[] = {
 
 static int usage(void) {
     fprintf(stderr,
-        "\nabpoa (B200): adaptive banded Partial Order Alignment, DP on the GPU (libabpoa_b200 %s)\n\n"
+        "\nabpoa (GPU): adaptive banded Partial Order Alignment, DP on the GPU (libabpoa_b200 %s)\n\n"
         "Usage: abpoa [options] <in.fa/fq> > cons.fa / msa.fa\n\n"
         "  -m --align-mode INT   0: global, 1: local, 2: extension [0]\n"
         "  -M --match INT / -X --mismatch INT / -t --matrix FILE   scores [2 / 4 / none]\n"

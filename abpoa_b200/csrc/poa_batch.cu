@@ -691,7 +691,7 @@ extern "C" int abpoa_gpu_msa_batch(abpoa_gpu_batch_t *e, abpoa_para_t *abpt, int
                                    abpoa_gpu_group_result_t *results, int flags) {
     if (n_groups <= 0) return 0;
     if (!((abpt->disable_seeding && abpt->progressive_poa == 0) || abpt->align_mode != ABPOA_GLOBAL_MODE))
-        poa_die(__func__, "minimizer seeding / guide-tree partitioning (-S / -p) is outside the scope of the B200 hot-path library.");
+        poa_die(__func__, "minimizer seeding / guide-tree partitioning (-S / -p) is outside the scope of the GPU hot-path library.");
     const auto t0 = std::chrono::steady_clock::now();
     /* ---- device-resident chain (poa_chain.cu): the whole progressive loop of a group runs on the GPU; whatever it
      *      cannot take (parameters outside its scope, groups that outgrow their slot) goes through the launch engine ---- */

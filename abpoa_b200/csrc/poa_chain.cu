@@ -405,8 +405,8 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         /* round index lists per cohort: wave-local slot indices of the groups that still have a read r */
         /* cohorts: each cohort's alignment kernel is one CTA (warp) per group; with at most one CTA per SM per cohort the
          * concurrently running kernels of all cohorts load every SM alike (a 250-CTA grid next to three more would put
-         * twice as many warps on the first 102 SMs as on the rest, and a round ends when its slowest warp does) */
-        int sm_count = 148; if (cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count < 1) sm_count = 148;
+         * twice as many warps on the first 118 SMs of an H100 as on the rest, and a round ends when its slowest warp does) */
+        int sm_count = 132; if (cudaDeviceGetAttribute(&sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sm_count < 1) sm_count = 132;
         const int auto_cohorts = std::max(1, std::min(16, (nw + sm_count - 1) / sm_count));
         const int use_cohorts = free_run ? 1 : (getenv("ABPOA_GPU_CHAIN_COHORTS") ? n_cohorts : auto_cohorts);
         std::vector<Cohort> coh((size_t)std::min(use_cohorts, nw));

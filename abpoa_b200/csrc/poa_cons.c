@@ -107,8 +107,8 @@ void abpoa_generate_consensus(abpoa_t *ab, abpoa_para_t *abpt) {
     abpoa_graph_t *abg = ab->abg;
     poa_graph_sync_public(abg);
     if (abg->is_called_cons == 1 || abg->node_n <= 2) return;
-    if (abpt->max_n_cons > 1) poa_die(__func__, "multi-consensus clustering (max_n_cons > 1) is outside the scope of the B200 hot-path library.");
-    if (abpt->cons_algrm != ABPOA_HB) poa_die(__func__, "most-frequent-base consensus is outside the scope of the B200 hot-path library.");
+    if (abpt->max_n_cons > 1) poa_die(__func__, "multi-consensus clustering (max_n_cons > 1) is outside the scope of the GPU hot-path library.");
+    if (abpt->cons_algrm != ABPOA_HB) poa_die(__func__, "most-frequent-base consensus is outside the scope of the GPU hot-path library.");
     cons_alloc(ab->abc, abg->node_n, ab->abs->n_seq, 1);
     heaviest_bundling(abg, ab->abc);
     abg->is_called_cons = 1;
@@ -220,12 +220,12 @@ void abpoa_output_rc_msa(abpoa_t *ab, abpoa_para_t *abpt, FILE *out_fp) {
 
 void abpoa_generate_gfa(abpoa_t *ab, abpoa_para_t *abpt, FILE *out_fp) {
     (void)ab; (void)abpt; (void)out_fp;
-    poa_die(__func__, "GFA output is outside the scope of the B200 hot-path library.");
+    poa_die(__func__, "GFA output is outside the scope of the GPU hot-path library.");
 }
 
 void abpoa_dump_pog(abpoa_t *ab, abpoa_para_t *abpt) {
     (void)ab; (void)abpt;
-    poa_die(__func__, "graph plotting is outside the scope of the B200 hot-path library.");
+    poa_die(__func__, "graph plotting is outside the scope of the GPU hot-path library.");
 }
 
 void abpoa_output(abpoa_t *ab, abpoa_para_t *abpt, FILE *out_fp) {

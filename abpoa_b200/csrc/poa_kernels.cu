@@ -1,4 +1,4 @@
-/* poa_kernels.cu -- sm_100a kernels for the adaptive-banded sequence-to-POA-graph DP
+/* poa_kernels.cu -- sm_90a kernels for the adaptive-banded sequence-to-POA-graph DP
  * and its backtrace.
  *
  * What is computed (the specification, validated cell-for-cell against the reference):

@@ -70,7 +70,7 @@ int abpoa_msa(abpoa_t *ab, abpoa_para_t *abpt, int n_seq, char **seq_names, int 
         fprintf(stderr, "[%s] Graph already exists, but incr_fn is also provided. Not restoring graph from file.\n", __func__);
     }
     if (!((abpt->disable_seeding && abpt->progressive_poa == 0) || abpt->align_mode != ABPOA_GLOBAL_MODE))
-        poa_die(__func__, "minimizer seeding / guide-tree partitioning (-S / -p) is outside the scope of the B200 hot-path library.");
+        poa_die(__func__, "minimizer seeding / guide-tree partitioning (-S / -p) is outside the scope of the GPU hot-path library.");
 
     const int exist_n_seq = abs->n_seq;
     abs->n_seq += n_seq; poa_seq_reserve(abs);
@@ -98,7 +98,7 @@ int abpoa_msa(abpoa_t *ab, abpoa_para_t *abpt, int n_seq, char **seq_names, int 
 extern char ab_char26_table[256];
 int abpoa_msa1(abpoa_t *ab, abpoa_para_t *abpt, char *read_fn, FILE *out_fp) {
     if (!abpt->out_msa && !abpt->out_cons && !abpt->out_gfa) return 0;
-    if (abpt->sort_input_seq) poa_die(__func__, "sorting the input by length (-L) is outside the scope of the B200 hot-path library.");
+    if (abpt->sort_input_seq) poa_die(__func__, "sorting the input by length (-L) is outside the scope of the GPU hot-path library.");
     abpoa_reset(ab, abpt, 1024);
     if (abpt->incr_fn) abpoa_restore_graph(ab, abpt);
     abpoa_seq_t *abs = ab->abs;
@@ -128,5 +128,5 @@ int abpoa_msa1(abpoa_t *ab, abpoa_para_t *abpt, char *read_fn, FILE *out_fp) {
 }
 abpoa_t *abpoa_restore_graph(abpoa_t *ab, abpoa_para_t *abpt) {
     (void)ab; (void)abpt;
-    poa_die(__func__, "restoring a graph from GFA/MSA files is outside the scope of the B200 hot-path library.");
+    poa_die(__func__, "restoring a graph from GFA/MSA files is outside the scope of the GPU hot-path library.");
 }

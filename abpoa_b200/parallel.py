@@ -102,7 +102,7 @@ def distributed_msa(groups, cfg, runner: Callable | None = None, balance: bool =
     """Run the MSA of every group on the ranks of the default process group.
 
     groups : list of read groups on rank 0 (ignored elsewhere).
-    runner : callable(cfg, list_of_groups) -> per group a list of numpy arrays; defaults to the B200 batch engine
+    runner : callable(cfg, list_of_groups) -> per group a list of numpy arrays; defaults to the GPU batch engine
              on the rank's current CUDA device, returning [consensus..., coverage...] per group.
     Returns the per-group results in input order on rank 0, None on the other ranks.
 

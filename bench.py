@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """bench.py -- GCUPS of the adaptive-banded sequence-to-POA-graph DP hot path.
 
-    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--groups G]
+    python bench.py --gpus N --steps K --warmup W [--impl reference] [--workload NAME] [--groups G] [--dump-outputs DIR]
 
 Workload (BASELINE.json configs[2], the one the metric is quoted on): synthetic read groups,
 50 reads x 10 kbp, 5 % ONT-like error, global alignment, convex gaps (-O 4,24 -E 2,1).
@@ -17,10 +17,12 @@ Printed JSON (rank 0):
             wall clock between barriers, max over ranks.
   roofline  dominant kernel (poa_align_kernel): algorithmic bytes = cells x S x (P + R x d) with
             the measured in-degree d, divided by the replay's kernel time, against the measured
-            HBM copy bandwidth in MEASURED_PEAKS.json.
+            HBM copy bandwidth in MEASURED_PEAKS.json (else the H100 SXM data sheet's 3.35 TB/s).
   cpu_baseline  the UNMODIFIED reference (oracle/_ref/libabpoa_ref.so, AVX2) on the host cores,
-            one process per physical core, on a bounded sample of the same groups.
+            one process per physical core, on a bounded sample of the same groups (null where the
+            reference has not been built).
 --impl reference prints the reference arm's line (CPU only; rank 0 alone runs).
+--dump-outputs DIR writes what the last timed step returned, rank 0's groups (see dump_outputs).
 """
 from __future__ import annotations
 
@@ -40,6 +42,8 @@ os.environ.setdefault("CUDA_MODULE_LOADING", "EAGER")
 
 ROOT = Path(__file__).resolve().parent
 sys.path.insert(0, str(ROOT))
+REF_LIB = ROOT / "oracle" / "_ref" / "libabpoa_ref.so"       # the unmodified reference, built by oracle/Makefile where its sources exist
+DUMP_BYTES = 64 << 20
 
 METRIC = "GCUPS (DP cells/s), global/convex 10 kbp"
 
@@ -106,7 +110,7 @@ def _ref_worker(args):
     from abpoa_b200 import capi, synth
     from abpoa_b200.aligner import PoaSession
     w = synth.WORKLOADS[wname]
-    lib = capi.load_library(ROOT / "oracle" / "_ref" / "libabpoa_ref.so")     # the unmodified reference (oracle/Makefile)
+    lib = capi.load_library(REF_LIB)
     cells = 0
     reads_done = 0
     groups = [synth.make_group(seed, n_reads, length, w.err, w.cfg.m) for seed in seeds]     # outside the timed window
@@ -165,7 +169,7 @@ def cpu_baseline_block(wname: str, w, ref_groups: int, base_seed: int) -> tuple[
 
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md recipe)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, index: int):
         self.index = index
@@ -206,7 +210,10 @@ def main():
     ap.add_argument("--groups", type=int, default=0, help="groups per GPU (default: the config's 1000)")
     ap.add_argument("--ref-groups", type=int, default=0, help="groups in one reference sample (default: one per core)")
     ap.add_argument("--no-cpu-baseline", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write the last timed step's results as DIR/<name>.npy")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
     if args.warmup < 3:
         args.warmup = 3
 
@@ -221,7 +228,7 @@ def main():
     cfgdesc = {"workload": f"{args.workload}: {n_groups} groups/GPU x {w.n_reads} reads x {w.length} bp, err {w.err}, "
                            f"{'global' if w.cfg.align_mode == 0 else 'local'}, O={w.cfg.gap_open1},{w.cfg.gap_open2} E={w.cfg.gap_ext1},{w.cfg.gap_ext2}",
                "groups_per_gpu": n_groups, "reads_per_group": w.n_reads, "read_len": w.length,
-               "l2_policy": "inputs larger than L2 (job blobs + DP planes of one step >> 126 MB)"}
+               "l2_policy": "inputs larger than L2 (job blobs + DP planes of one step >> 50 MB)"}
 
     # ---------------------------------------------------------------- reference arm
     if args.impl == "reference":
@@ -260,7 +267,7 @@ def main():
         }))
         return
 
-    # ---------------------------------------------------------------- B200 arm
+    # ---------------------------------------------------------------- GPU arm
     import torch
     import torch.distributed as dist
     torch.cuda.set_device(local_rank)
@@ -303,8 +310,12 @@ def main():
     t0 = time.perf_counter()
     cells = 0
     cons_bases = 0
-    for _ in range(args.steps):
-        res = eng.run_packed(abpt, packed, keep_results=False)
+    for step in range(args.steps):
+        if args.dump_outputs and rank == 0 and step == args.steps - 1:
+            last = eng.run_packed(abpt, packed, keep_results=True)
+            res = [(r.dp_cells, r.n_aligned, sum(len(c) for c in r.cons)) for r in last]
+        else:
+            res = eng.run_packed(abpt, packed, keep_results=False)
         cells += sum(r[0] for r in res)
         cons_bases += sum(r[2] for r in res)
     barrier()
@@ -328,7 +339,7 @@ def main():
     # engine, upload once, replay back to back with CUDA-event timing (per-launch numbers for the roofline)
     eng.run_packed(abpt, packed, keep_results=False, capture=True)
     barrier()
-    rp = eng.replay(abpt, warmup=1, repeats=max(args.steps, 2))
+    rp = eng.replay(abpt, warmup=1, repeats=args.steps)
     eng.clear_capture()
     kt = torch.tensor([rp["kernel_ms"]], dtype=torch.float64, device="cuda")
     kc = torch.tensor([float(rp["cells"])], dtype=torch.float64, device="cuda")
@@ -360,7 +371,7 @@ def main():
 
     # parity sample: consensus of the first groups of rank 0 against the reference's (computed in the cpu_baseline leg)
     sample_cons = None
-    if rank == 0 and not args.no_cpu_baseline and world == 1:
+    if rank == 0 and not args.no_cpu_baseline and world == 1 and REF_LIB.exists():
         k = min(n_groups, args.ref_groups or len([c_ for v in socket_cpus().values() for c_ in v]))
         sub = PackedGroups(groups[:k])
         sample_cons = [bytes(r.cons[0]) if r.cons else b"" for r in eng.run_packed(abpt, sub, keep_results=True)]
@@ -383,22 +394,8 @@ def main():
         peak = json.loads(peaks_file.read_text())["hbm_gbs"]
         peak_src = "measured (MEASURED_PEAKS.json hbm_gbs)"
     else:
-        peak, peak_src = 6650.0, "fallback (B200_PROFILING.md)"
-    # DRAM bytes of one launch of the dominant kernel from the committed `ncu --set full` capture (profiles/)
-    traffic, traffic_note, dram_frac = None, None, None
-    gapname = {1: "linear", 3: "affine", 5: "convex"}[P]
-    for cand in (ROOT / "profiles" / f"r02_ncu_traffic_{gapname}.json", ROOT / "profiles" / "r01_ncu_traffic.json"):
-        if cand.exists():
-            t_ = json.loads(cand.read_text())
-            if cand.name.startswith("r01") and P != 5:
-                continue
-            traffic = t_["dram_bytes_read"] + t_["dram_bytes_write"]
-            dram_frac = traffic / (t_["duration_ms"] / 1e3) / 1e9 / peak
-            traffic_note = (f"ncu capture of one launch of {t_.get('kernel', 'the kernel').split('(')[0]} ({t_['jobs']} jobs, {t_['duration_ms']:.1f} ms): "
-                            f"{t_['dram_bytes_write'] / 1e9:.1f} GB written + {t_['dram_bytes_read'] / 1e9:.1f} GB read; see {t_['source']}")
-            break
-    roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak, "traffic": traffic, "traffic_note": traffic_note,
-                "dram_frac_measured": dram_frac,
+        peak, peak_src = 3350.0, "H100 SXM data sheet (HBM3), not measured"
+    roofline = {"bound": "hbm", "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
                 "kernel": "poa_align_kernel_p16 / poa_chain_align_kernel_p16 (same job function)", "bytes_per_cell": (bytes16 + bytes32) / max(rp["cells"], 1), "mean_in_degree": d,
                 "peak_source": peak_src, "launches_per_pass": rp["launches"], "replay_mismatches": rp["mismatches"],
                 "int16_cell_fraction": rp["cells16"] / max(rp["cells"], 1), "kernel_alone_gcups": kernel_only_gcups,
@@ -406,7 +403,7 @@ def main():
 
     cpu = None
     parity = None
-    if not args.no_cpu_baseline and world == 1:        # N=1 only (the contract); workers are pinned over ALL cores of the box
+    if not args.no_cpu_baseline and world == 1 and REF_LIB.exists():        # N=1 only; workers are pinned over ALL cores of the box
         cpu, ref_run = cpu_baseline_block(args.workload, w, args.ref_groups, 1000)
         if sample_cons is not None:                    # rank 0's groups g = seed 1000 + g: the very groups the reference just ran
             same = sum(1 for g, cb in enumerate(sample_cons) if ref_run["cons"].get(1000 + g) == cb)
@@ -446,9 +443,32 @@ def main():
         "kernel_only": {"ms_per_pass": rp["kernel_ms"], "ms_min": rp["kernel_ms_min"], "jobs": rp["n_jobs"], "cells": rp["cells"], "hbm_resident_input_bytes": rp["input_bytes"],
                         "gcups": kernel_only_gcups},
     }))
+    if args.dump_outputs:
+        dump_outputs(Path(args.dump_outputs), last)
     eng.close()
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(out: Path, results) -> None:
+    """What abpoa_gpu_msa_batch returned for rank 0's groups in the last timed step, as float64 / float32 .npy files:
+    per group DP cells, aligned reads and consensus length, and the consensus bases and coverage of every group -- or,
+    when those exceed the size budget, of a fixed seeded sample of groups (sample_groups.npy)."""
+    import numpy as np
+    out.mkdir(parents=True, exist_ok=True)
+    n = len(results)
+    np.save(out / "group_dp_cells.npy", np.array([r.dp_cells for r in results], dtype=np.float64))
+    np.save(out / "group_n_aligned.npy", np.array([r.n_aligned for r in results], dtype=np.float64))
+    np.save(out / "consensus_len.npy", np.array([sum(len(c) for c in r.cons) for r in results], dtype=np.float64))
+    total = sum(len(c) for r in results for c in r.cons)
+    budget = (DUMP_BYTES * 9 // 10 - 8 * 4 * n) // 8        # consensus + coverage, 4 bytes each per base; slack for sampled groups longer than the mean
+    pick = np.arange(n)
+    if total > budget:
+        pick = np.sort(np.random.default_rng(0).choice(n, size=max(1, n * budget // total), replace=False))
+    np.save(out / "sample_groups.npy", pick.astype(np.float64))
+    cat = lambda xs: np.concatenate(xs).astype(np.float32) if xs else np.zeros(0, dtype=np.float32)
+    np.save(out / "consensus.npy", cat([c for g in pick for c in results[g].cons]))
+    np.save(out / "coverage.npy", cat([c for g in pick for c in results[g].cov]))
 
 
 if __name__ == "__main__":

@@ -1,4 +1,4 @@
-/* abpoa.h -- public C ABI of the B200-native POA engine (libabpoa_b200.so).
+/* abpoa.h -- public C ABI of the H100-native POA engine (libabpoa_b200.so).
  *
  * This header is the DROP-IN BOUNDARY: it declares, with identical names, argument
  * order, struct layouts and constants, the C interface that abPOA v1.5.6 exposes in
@@ -6,7 +6,7 @@
  * :150-230 functions).  A program compiled against the reference header links and
  * runs against this library unchanged; the sequence-to-graph dynamic program that
  * the reference runs on SSE/AVX (src/abpoa_align_simd.c) is executed here by
- * hand-written sm_100a CUDA kernels.
+ * hand-written sm_90a CUDA kernels.
  *
  * Differences that are invisible to callers:
  *   - the reference includes simd_instruction.h only to name `SIMDi*` for the opaque

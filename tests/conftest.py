@@ -16,7 +16,7 @@ os.environ.setdefault("ABPOA_GPU_CHECK_ORDER", "1")     # the whole suite runs w
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device")
 
 
 @pytest.fixture(scope="session")
@@ -25,12 +25,10 @@ def product_lib():
     return capi.product()
 
 
-REFERENCE_LIB = ROOT / "oracle" / "_ref" / "libabpoa_ref.so"      # the unmodified reference, built by oracle/Makefile
-
-
 @pytest.fixture(scope="session")
-def reference_lib():
-    from abpoa_b200 import capi
-    if not REFERENCE_LIB.exists():
-        pytest.skip("oracle/_ref/libabpoa_ref.so not built (reference tree absent and no prebuilt copy)")
-    return capi.load_library(REFERENCE_LIB)
+def reference():
+    """The unmodified reference's results on the parity inputs (tests/reference_runs.py)."""
+    from reference_runs import Reference
+    ref = Reference()
+    yield ref
+    ref.save()

@@ -8,7 +8,6 @@ import numpy as np
 from abpoa_b200.aligner import PoaConfig, PoaSession, encode
 
 INPUTS = Path(__file__).resolve().parent / "golden" / "inputs"
-REFERENCE_LIB = Path(__file__).resolve().parent.parent / "oracle" / "_ref" / "libabpoa_ref.so"
 
 
 def read_fasta(path: Path, m: int = 5) -> list[np.ndarray]:
@@ -70,26 +69,6 @@ def run_group(lib, cfg: PoaConfig, reads, want_msa: bool = True, use_oracle: boo
         }
 
 
-def assert_group_equal(a, b, tag=""):
-    assert len(a["alns"]) == len(b["alns"])
-    for i, (x, y) in enumerate(zip(a["alns"], b["alns"])):
-        assert x.aligned == y.aligned, f"{tag} read {i}: aligned flag"
-        if not x.aligned:
-            continue
-        assert x.best_score == y.best_score, f"{tag} read {i}: best_score {x.best_score} != {y.best_score}"
-        assert x.cigar.shape == y.cigar.shape and np.array_equal(x.cigar, y.cigar), f"{tag} read {i}: graph_cigar differs"
-        assert (x.node_s, x.node_e, x.query_s, x.query_e) == (y.node_s, y.node_e, y.query_s, y.query_e), f"{tag} read {i}: ends"
-        assert x.cells == y.cells, f"{tag} read {i}: DP cells {x.cells} != {y.cells}"
-    assert len(a["cons"]) == len(b["cons"])
-    for x, y in zip(a["cons"], b["cons"]):
-        assert np.array_equal(x, y), f"{tag}: consensus differs"
-    for x, y in zip(a["cov"], b["cov"]):
-        assert np.array_equal(x, y), f"{tag}: consensus coverage differs"
-    assert len(a["msa"]) == len(b["msa"])
-    for x, y in zip(a["msa"], b["msa"]):
-        assert np.array_equal(x, y), f"{tag}: RC-MSA differs"
-
-
 def group_digest(r, m: int = 5):
     """Same shape as the entries of tests/golden/golden.json."""
     import hashlib
@@ -114,27 +93,3 @@ def assert_digest_equal(got, want, tag=""):
         assert x == y, f"{tag} read {i}: {x} != {y}"
     for k in ("cons", "cov_sha1", "msa_len", "msa_sha1"):
         assert got[k] == want[k], f"{tag}: {k} differs"
-
-
-def _ref_records_worker(args):
-    """(spawned process) one group through the unmodified reference: per-read score / CIGAR length /
-    FNV-1a hash of the CIGAR words / DP cells, consensus, coverage."""
-    cfg_kw, reads, want_msa = args
-    from abpoa_b200 import capi
-    from abpoa_b200.batch import fnv1a_words
-    r = run_group(capi.load_library(REFERENCE_LIB), PoaConfig(**cfg_kw), reads, want_msa=want_msa)
-    return {
-        "score": [a.best_score if a.aligned else 0 for a in r["alns"]],
-        "n_cigar": [len(a.cigar) for a in r["alns"]],
-        "hash": [fnv1a_words(a.cigar) if a.aligned else None for a in r["alns"]],
-        "cells": sum(a.cells for a in r["alns"]),
-        "cons": r["cons"], "cov": r["cov"], "msa": r["msa"],
-    }
-
-
-def reference_records(cfg: PoaConfig, groups, want_msa=False, procs=4):
-    """Run the groups through oracle/_ref in parallel worker processes (the reference is single-threaded and,
-    at 10 kbp, page-fault bound: ~15 s per 50-read group)."""
-    import multiprocessing as mp
-    with mp.get_context("spawn").Pool(min(procs, len(groups))) as pool:
-        return pool.map(_ref_records_worker, [(dict(cfg.__dict__), g, want_msa) for g in groups])

@@ -1,19 +1,11 @@
-"""Drop-in boundary against the REFERENCE's own files (CPU; skipped where /root/reference does not exist, e.g. on the GPU box):
-
-* struct layout: a probe compiled once against /root/reference/include/abpoa.h and once against include/abpoa.h must print the
-  same sizeof / offsetof for every public struct and the same values for every constant;
-* the reference's example programs (example.c, sub_example.c, incre_example.c) compile against OUR header and link against
-  libabpoa_b200.so unchanged (running them needs a GPU; on a GPU box the library's own tests cover the same calls)."""
+"""Drop-in boundary against the reference's public header: a probe compiled against include/abpoa.h must print the
+same sizeof / offsetof for every public struct and the same values for every constant as the same probe compiled
+against the reference's include/abpoa.h (abPOA v1.5.6, x86-64, gcc), stored in tests/golden/reference_abi.txt."""
 import subprocess
 from pathlib import Path
 
-import pytest
-
 ROOT = Path(__file__).resolve().parent.parent
-REF = Path("/root/reference")
-LIBDIR = ROOT / "abpoa_b200" / "lib"
-
-pytestmark = pytest.mark.skipif(not (REF / "include" / "abpoa.h").exists(), reason="reference tree not present")
+GOLDEN = Path(__file__).resolve().parent / "golden" / "reference_abi.txt"
 
 PROBE = r'''
 #include <stdio.h>
@@ -57,15 +49,5 @@ def probe(tmp_path, tag, include_dirs):
 
 def test_public_structs_match_the_reference_header(tmp_path):
     ours = probe(tmp_path, "ours", [ROOT / "include"])
-    theirs = probe(tmp_path, "ref", [REF / "include"])
+    theirs = GOLDEN.read_text()
     assert ours == theirs, "\n".join(f"{a}   |   {b}" for a, b in zip(ours.splitlines(), theirs.splitlines()) if a != b)
-
-
-@pytest.mark.parametrize("prog", ["example.c", "sub_example.c", "incre_example.c"])
-def test_reference_examples_build_against_this_library(tmp_path, prog):
-    if not (LIBDIR / "libabpoa_b200.so").exists():
-        pytest.skip("library not built")
-    exe = tmp_path / prog.replace(".c", "")
-    r = subprocess.run(["gcc", "-O1", "-w", f"-I{ROOT / 'include'}", "-o", str(exe), str(REF / prog), f"-L{LIBDIR}", "-labpoa_b200", f"-Wl,-rpath,{LIBDIR}", "-lm", "-lz", "-lpthread"],
-                       capture_output=True, text=True)
-    assert r.returncode == 0, r.stderr

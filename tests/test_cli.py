@@ -3,7 +3,7 @@
 CPU part: the reader (poa_read_fastx, grammar of the reference's kseq-based abpoa_read_seq) on the reference's own
 test inputs, plain and gzip-compressed.  GPU part: the real binary reproduces the md5 vectors recorded from the
 reference CLI (SURVEY 8c / tests/golden/golden.json) and, in list mode (-l: all files as ONE GPU batch), prints
-byte for byte what the reference binary prints for the same list."""
+byte for byte what the reference binary prints for the same list (md5 stored by tests/reference_runs.py)."""
 import ctypes as C
 import gzip
 import hashlib
@@ -19,7 +19,7 @@ from helpers import INPUTS
 
 ROOT = Path(__file__).resolve().parent.parent
 BIN = ROOT / "abpoa_b200" / "bin" / "abpoa"
-REF_BIN = ROOT / "oracle" / "_ref" / "abpoa_ref"
+REF_BIN = ROOT / "oracle" / "_ref" / "abpoa_ref"      # the reference CLI (oracle/Makefile), for recording
 
 
 def read_with_library(lib, path):
@@ -78,8 +78,8 @@ def test_fastx_reader_multiline_and_crlf(product_lib, tmp_path):
     assert read_with_library(product_lib, p) == [("r1", "first read", "ACGTAC", ""), ("r2", "", "GGTTA", ""), ("r3", "x y", "C", "")]
 
 
-def md5_of(args):
-    out = subprocess.run([str(BIN), *args], capture_output=True, check=True).stdout
+def md5_of(args, binary=BIN):
+    out = subprocess.run([str(binary), *args], capture_output=True, check=True).stdout
     return hashlib.md5(out).hexdigest()
 
 
@@ -102,11 +102,9 @@ def test_cli_md5_vector_test_fa():
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("opts", [[], ["-r1"], ["-r2"], ["-r5"], ["-m", "1", "-r2"], ["-Q", "-r2"]])
-def test_cli_list_mode_matches_reference_binary(tmp_path, opts):
+def test_cli_list_mode_matches_reference_binary(reference, tmp_path, opts):
     """-l: every file is one read group; ours runs them as one GPU batch (device chain for consensus output, launch
     engine otherwise) and must print what the reference prints file by file."""
-    if not REF_BIN.exists():
-        pytest.skip("oracle/_ref/abpoa_ref not built")
     files = []
     for g in range(7):
         reads = synth.make_group(7000 + g, 4 + g % 4, 150 + 60 * g, 0.06)
@@ -117,6 +115,6 @@ def test_cli_list_mode_matches_reference_binary(tmp_path, opts):
     files.append(INPUTS / "heter.fq")
     lst = tmp_path / "list.txt"
     lst.write_text("".join(f"{p}\n" for p in files))
-    ours = subprocess.run([str(BIN), *opts, "-l", str(lst)], capture_output=True, check=True).stdout
-    ref = subprocess.run([str(REF_BIN), *opts, "-l", str(lst)], capture_output=True, check=True).stdout
-    assert ours == ref
+    inputs = [hashlib.sha1(p.read_bytes()).hexdigest() for p in files]
+    ref = reference.value("cli_list", (opts, inputs), lambda: md5_of([*opts, "-l", str(lst)], REF_BIN))
+    assert md5_of([*opts, "-l", str(lst)]) == ref

@@ -3,7 +3,7 @@
 * single-alignment path (abpoa.h: abpoa_align_sequence_to_graph + abpoa_add_graph_alignment) against
   the golden vectors generated from the unmodified reference (tests/golden/golden.json) -- no oracle,
   no reference library involved: per-read score, CIGAR sha1, end points, DP cells, consensus, RC-MSA;
-* batch engine (abpoa_gpu.h) against the live reference (oracle/_ref) with per-read CIGAR hashes;
+* batch engine (abpoa_gpu.h) against the reference's results (tests/reference_runs.py) with per-read CIGAR hashes;
 * every fallback of the launcher forced through environment switches: generic int16 kernel
   (ABPOA_GPU_NO_P16), range guard of the packed kernel (ABPOA_GPU_FORCE_P16 on a case that needs 32
   bits), plane-slab overflow redo (ABPOA_GPU_SLAB_PCT), Kahn order instead of the spliced order
@@ -23,7 +23,8 @@ from abpoa_b200.aligner import PoaConfig, PoaSession
 from abpoa_b200.batch import BatchEngine, fnv1a_words
 from abpoa_b200.capi import abpoa_res_t, c_u8_p
 from cases import AFFINE, CASES, case_reads, case_weights
-from helpers import assert_digest_equal, assert_group_equal, group_digest, run_group
+from helpers import assert_digest_equal, group_digest, run_group
+from reference_runs import Hasher, assert_batch_matches, assert_run_matches
 
 pytestmark = pytest.mark.gpu
 
@@ -73,7 +74,7 @@ def run_group_counting_retries(lib, cfg, reads):
         return {"alns": alns, "cons": s.consensus(), "cov": s.consensus_cov(), "msa": s.msa_rows(), "order_stats": None}, _retries(s)
 
 
-def test_range_guard_redo(product_lib, reference_lib, monkeypatch):
+def test_range_guard_redo(product_lib, reference, monkeypatch):
     """Scores that really leave the int16 window (2 kbp x match 20 = 40 000), forced onto the packed int16 kernel: its
     run-time guard must report POA_ST_RANGE and the 32-bit redo must give the reference's result."""
     monkeypatch.setenv("ABPOA_GPU_FORCE_P16", "1")
@@ -81,7 +82,7 @@ def test_range_guard_redo(product_lib, reference_lib, monkeypatch):
     reads = synth.make_group(31, 6, 2000, 0.05)
     got, retries = run_group_counting_retries(product_lib, cfg, reads)
     assert retries > 0, "the packed kernel never reported RANGE on scores beyond int16"
-    assert_group_equal(got, run_group(reference_lib, cfg, reads), "range-redo")
+    assert_run_matches(got, reference.run(cfg, reads), "range-redo")
 
 
 @pytest.mark.parametrize("name", ["syn_convex_2k", "syn_affine_1k", "syn_high_error"])
@@ -96,29 +97,17 @@ def test_plane_overflow_redo(product_lib, monkeypatch, name):
 
 
 # ------------------------------------------------------------------------------------------- batch engine
-def check_batch(reference_lib, cfg, groups, weights=None, cells=True, **engine_kw):
+def check_batch(reference, cfg, groups, weights=None, **engine_kw):
     with BatchEngine(**engine_kw) as eng:
         got = eng.run(cfg, groups, record_reads=True, weights=weights)
         st = eng.stats()
     assert st["alignments"] >= sum(max(len(g) - 1, 0) for g in groups)
-    for gi, (g, r) in enumerate(zip(groups, got)):
-        ref = run_group(reference_lib, cfg, g, want_msa=cfg.out_msa, weights=weights[gi] if weights else None)
-        if cells:
-            assert r.dp_cells == sum(a.cells for a in ref["alns"]), f"group {gi}: cells"
-        for i, a in enumerate(ref["alns"]):
-            if not a.aligned:
-                continue
-            assert r.read_best_score[i] == a.best_score, f"group {gi} read {i}: score"
-            assert r.read_n_cigar[i] == len(a.cigar), f"group {gi} read {i}: n_cigar"
-            assert int(r.read_cigar_hash[i]) == fnv1a_words(a.cigar), f"group {gi} read {i}: cigar hash"
-        assert len(r.cons) == len(ref["cons"]) and all(np.array_equal(x, y) for x, y in zip(r.cons, ref["cons"])), f"group {gi}: consensus"
-        assert all(np.array_equal(x, y) for x, y in zip(r.cov, ref["cov"])), f"group {gi}: coverage"
-        assert len(r.msa) == len(ref["msa"]) and all(np.array_equal(x, y) for x, y in zip(r.msa, ref["msa"])), f"group {gi}: msa"
+    assert_batch_matches(got, groups, reference.batch(cfg, groups, want_msa=cfg.out_msa, weights=weights))
     return st
 
 
 @pytest.mark.parametrize("name", list(CASES))
-def test_case_batch_engine(reference_lib, name):
+def test_case_batch_engine(reference, name):
     """The same cases through abpoa_gpu_msa_batch (two groups: the case's reads, and the same reads in
     reverse order so that the groups differ), alternately consensus-only and with the RC-MSA."""
     case = CASES[name]
@@ -128,31 +117,31 @@ def test_case_batch_engine(reference_lib, name):
     w = case_weights(case, reads)
     groups = [reads, reads[::-1]]
     weights = [w, w[::-1]] if w is not None else None
-    check_batch(reference_lib, cfg, groups, weights=weights, n_workers=2, groups_per_launch=1)
+    check_batch(reference, cfg, groups, weights=weights, n_workers=2, groups_per_launch=1)
 
 
-def test_batch_exact_order(reference_lib, monkeypatch):
+def test_batch_exact_order(reference, monkeypatch):
     """ABPOA_GPU_EXACT_ORDER=1: the reference's Kahn order after every read instead of the spliced order."""
     monkeypatch.setenv("ABPOA_GPU_EXACT_ORDER", "1")
     groups = [synth.make_group(1300 + g, 6, 500, 0.08) for g in range(6)]
-    check_batch(reference_lib, PoaConfig(), groups, n_workers=2, groups_per_launch=2)
+    check_batch(reference, PoaConfig(), groups, n_workers=2, groups_per_launch=2)
 
 
-def test_batch_arena_contention(reference_lib, monkeypatch):
+def test_batch_arena_contention(reference, monkeypatch):
     """A plane arena that holds only a few launches: sub-chunks must take the drain-then-block path
     (no worker waits for planes while holding some) and still deliver every group."""
     monkeypatch.setenv("ABPOA_GPU_ARENA_MB", "4")
     groups = [synth.make_group(1500 + g, 8, 300 + 20 * (g % 5), 0.05) for g in range(64)]
-    check_batch(reference_lib, PoaConfig(**AFFINE), groups, n_workers=4, groups_per_launch=4)
+    check_batch(reference, PoaConfig(**AFFINE), groups, n_workers=4, groups_per_launch=4)
 
 
-def test_batch_no_p16_and_slab_redo(reference_lib, monkeypatch):
+def test_batch_no_p16_and_slab_redo(reference, monkeypatch):
     """Redo paths inside the pipelined engine (poa_engine_collect): slab overflow on the generic kernel (with the packed
     kernel switched off the chain engine, which only has that kernel, steps aside)."""
     monkeypatch.setenv("ABPOA_GPU_NO_P16", "1")
     monkeypatch.setenv("ABPOA_GPU_SLAB_PCT", "30")
     groups = [synth.make_group(1700 + g, 6, 400, 0.06) for g in range(10)]
-    st = check_batch(reference_lib, PoaConfig(), groups, n_workers=2, groups_per_launch=3)
+    st = check_batch(reference, PoaConfig(), groups, n_workers=2, groups_per_launch=3)
     assert st["retries"] > 0
 
 
@@ -165,24 +154,27 @@ def deletion_fan(seed=7, n=40, flank=220):
     return [t] + [np.concatenate([t[: flank - k], t[flank:]]) for k in range(1, n)]
 
 
-@pytest.mark.parametrize("gap", ["convex", "affine"])
-def test_more_than_32_predecessors(product_lib, reference_lib, gap):
-    cfg = PoaConfig(**(AFFINE if gap == "affine" else {}))
-    reads = deletion_fan()
-    ref = run_group(reference_lib, cfg, reads)
-    with PoaSession(cfg, reference_lib) as s:
+def max_in_degree(lib, cfg, reads):
+    with PoaSession(cfg, lib) as s:
         s.run_reads(reads, count_cells=False)
         g = s.ab.contents.abg.contents
-        deg = max(g.node[i].in_edge_n for i in range(g.node_n))
+        return max(g.node[i].in_edge_n for i in range(g.node_n))
+
+
+@pytest.mark.parametrize("gap", ["convex", "affine"])
+def test_more_than_32_predecessors(product_lib, reference, gap):
+    cfg = PoaConfig(**(AFFINE if gap == "affine" else {}))
+    reads = deletion_fan()
+    deg = reference.value("max_in_degree", gap, lambda: max_in_degree(reference.lib, cfg, reads), reads)
     assert deg > 32, f"the construction only reached in-degree {deg}"
-    assert_group_equal(run_group(product_lib, cfg, reads), ref, f"fan/{gap}")
+    assert_run_matches(run_group(product_lib, cfg, reads), reference.run(cfg, reads), f"fan/{gap}")
 
 
-def test_more_than_32_predecessors_generic_kernel(product_lib, reference_lib, monkeypatch):
+def test_more_than_32_predecessors_generic_kernel(product_lib, reference, monkeypatch):
     monkeypatch.setenv("ABPOA_GPU_NO_P16", "1")
     cfg = PoaConfig()
     reads = deletion_fan(seed=8)
-    assert_group_equal(run_group(product_lib, cfg, reads), run_group(reference_lib, cfg, reads), "fan/generic")
+    assert_run_matches(run_group(product_lib, cfg, reads), reference.run(cfg, reads), "fan/generic")
 
 
 # ------------------------------------------------------------------------------------------- -s and sub-graphs
@@ -195,33 +187,33 @@ def strand_mix(seed, n, length):
 
 
 def msa_whole(lib, cfg, reads):
+    """abpoa_msa over the whole group: which reads were flipped, and a digest of the consensus and RC-MSA."""
     with PoaSession(cfg, lib) as s:
         s.msa(reads)
         abs_ = s.ab.contents.abs.contents
         is_rc = [int(abs_.is_rc[i]) for i in range(len(reads))]
-        return {"cons": s.consensus(), "cov": s.consensus_cov(), "msa": s.msa_rows(), "is_rc": is_rc}
+        return {"is_rc": is_rc, "cons_msa": Hasher().arrays(s.consensus()).arrays(s.msa_rows()).hex()}
 
 
-def test_amb_strand_msa(product_lib, reference_lib):
+def test_amb_strand_msa(product_lib, reference):
     """abpoa_msa with -s (reference src/abpoa_align.c:323-344): weak forward hits are re-aligned as reverse complement."""
     cfg = PoaConfig(amb_strand=True, out_msa=True)
     reads = strand_mix(1900, 9, 600)
-    a, b = msa_whole(product_lib, cfg, reads), msa_whole(reference_lib, cfg, reads)
+    a = msa_whole(product_lib, cfg, reads)
+    b = reference.value("msa_whole", "amb_strand", lambda: msa_whole(reference.lib, cfg, reads), reads)
     assert sum(b["is_rc"]) >= 2, "the reference flipped no read: the case does not exercise -s"
     assert a["is_rc"] == b["is_rc"]
-    assert all(np.array_equal(x, y) for x, y in zip(a["cons"], b["cons"]))
-    assert len(a["msa"]) == len(b["msa"]) and all(np.array_equal(x, y) for x, y in zip(a["msa"], b["msa"]))
+    assert a["cons_msa"] == b["cons_msa"], "consensus or RC-MSA differs from the reference"
 
 
-def test_amb_strand_batch(product_lib, reference_lib):
+def test_amb_strand_batch(product_lib, reference):
     cfg = PoaConfig(amb_strand=True, out_msa=True)
     groups = [strand_mix(1950 + g, 7, 400 + 50 * g) for g in range(5)]
     with BatchEngine(n_workers=2, groups_per_launch=2) as eng:
         got = eng.run(cfg, groups)
     for gi, (g, r) in enumerate(zip(groups, got)):
-        ref = msa_whole(reference_lib, cfg, g)
-        assert all(np.array_equal(x, y) for x, y in zip(r.cons, ref["cons"])), f"group {gi}: consensus"
-        assert len(r.msa) == len(ref["msa"]) and all(np.array_equal(x, y) for x, y in zip(r.msa, ref["msa"])), f"group {gi}: msa"
+        ref = reference.value("msa_whole", "amb_strand", lambda: msa_whole(reference.lib, cfg, g), g)
+        assert Hasher().arrays(r.cons).arrays(r.msa).hex() == ref["cons_msa"], f"group {gi}: consensus or msa"
 
 
 def subgraph_walk(lib, cfg, reads, windows):
@@ -250,11 +242,14 @@ def subgraph_walk(lib, cfg, reads, windows):
             if res.n_cigar > 0:
                 capi.libc_free(res.graph_cigar)
         s.generate()
-        return out, s.consensus(), s.msa_rows()
+        h = Hasher()
+        for rc, eb_, ee_, score, cig, ends in out:
+            h.add((rc, eb_, ee_, score, ends)).arrays([cig.view(np.int64)])
+        return h.arrays(s.consensus()).arrays(s.msa_rows()).hex()
 
 
 @pytest.mark.parametrize("path_score", [False, True])
-def test_subgraph_alignment(product_lib, reference_lib, path_score):
+def test_subgraph_alignment(product_lib, reference, path_score):
     """Sub-graph windows (the index_map / live-row filter of the DP entry, reference
     src/abpoa_align_simd.c:1257-1269), with and without -G, whose score lookup uses the filtered index."""
     rng = np.random.default_rng(77)
@@ -269,19 +264,14 @@ def test_subgraph_alignment(product_lib, reference_lib, path_score):
         reads.append(piece)
         windows.append((2 + a, 2 + b - 1))   # the first read's base i became node id 2 + i
     cfg = PoaConfig(inc_path_score=path_score, out_msa=True)
-    a = subgraph_walk(product_lib, cfg, reads, windows)
-    b = subgraph_walk(reference_lib, cfg, reads, windows)
-    for i, (x, y) in enumerate(zip(a[0], b[0])):
-        assert x[:4] == y[:4], f"read {i}: rc / window / score {x[:4]} vs {y[:4]}"
-        assert np.array_equal(x[4], y[4]), f"read {i}: graph-CIGAR"
-        assert x[5] == y[5], f"read {i}: ends"
-    assert all(np.array_equal(x, y) for x, y in zip(a[1], b[1]))
-    assert len(a[2]) == len(b[2]) and all(np.array_equal(x, y) for x, y in zip(a[2], b[2]))
+    want = reference.value("subgraph_walk", (path_score, windows), lambda: subgraph_walk(reference.lib, cfg, reads, windows), reads)
+    assert subgraph_walk(product_lib, cfg, reads, windows) == want, \
+        "return codes, windows, scores, graph-CIGARs, end points, consensus or RC-MSA differ from the reference"
 
 
 # ------------------------------------------------------------------------------------------- a7: banded linear gaps, lane-exact
 @pytest.mark.parametrize("mode", [0, 2])
-def test_linear_banded_lane_exact_sweep(product_lib, reference_lib, mode):
+def test_linear_banded_lane_exact_sweep(product_lib, reference, mode):
     """Banded linear-gap alignment (global and extend): the specification is the reference's vector procedure (SURVEY 8a a7:
     leaked cells right of `end`, vector-granular predecessor reads, incomplete scans beyond the predecessors' last vector).
     Sweep of group shapes, error rates (3-25 %) and band widths: every score, graph-CIGAR word, end point AND the DP-cell
@@ -292,15 +282,14 @@ def test_linear_banded_lane_exact_sweep(product_lib, reference_lib, mode):
         reads = synth.make_group(5000 + seed, 4 + seed % 5, 150 + 37 * (seed % 9), [0.03, 0.08, 0.15, 0.25][seed % 4])
         cfg = PoaConfig(align_mode=mode, **LINEAR) if seed % 2 == 0 else PoaConfig(align_mode=mode, wb=6 + seed % 7, wf=0.01, **LINEAR)
         a = run_group(product_lib, cfg, reads)
-        b = run_group(reference_lib, cfg, reads)
-        assert_group_equal(a, b, f"linear banded mode {mode} seed {seed}")
+        assert_run_matches(a, reference.run(cfg, reads), f"linear banded mode {mode} seed {seed}")
         n_aln += sum(1 for x in a["alns"] if x.aligned)
     assert n_aln >= 250
 
 
-def test_linear_banded_int32_width(product_lib, reference_lib):
+def test_linear_banded_int32_width(product_lib, reference):
     """The same with scores that make the reference pick int32 (vectors of 8 lanes instead of 16)."""
     cfg = PoaConfig(match=20, mismatch=40, gap_open1=0, gap_ext1=20, gap_open2=0, gap_ext2=0, wb=8)
     for seed in range(6):
         reads = synth.make_group(5100 + seed, 6, 1800, 0.10)
-        assert_group_equal(run_group(product_lib, cfg, reads), run_group(reference_lib, cfg, reads), f"linear banded int32 seed {seed}")
+        assert_run_matches(run_group(product_lib, cfg, reads), reference.run(cfg, reads), f"linear banded int32 seed {seed}")

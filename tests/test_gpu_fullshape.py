@@ -1,58 +1,44 @@
 """GPU parity at the BENCHMARKED sizes (BASELINE.json configs 2-5), product vs the unmodified
-reference (oracle/_ref): per-read best score, graph-CIGAR length and FNV-1a hash of every CIGAR word,
-DP-cell totals, consensus and coverage.
+reference (stored by tests/reference_runs.py): per-read best score, graph-CIGAR length and FNV-1a
+hash of every CIGAR word, DP-cell totals, consensus and coverage.
 
 Small cases cannot reach what these do: 25 k-row graphs, bands wider than one 256-cell pass, scores
 close to the packed kernel's int16 window, graphs past the point where the reference itself switches
 to int32 (gn > 16 364), 20-pass rows in local mode.
 """
-import numpy as np
 import pytest
 
 from abpoa_b200 import synth
 from abpoa_b200.batch import BatchEngine
-from helpers import reference_records
+from reference_runs import assert_batch_matches
 
 pytestmark = pytest.mark.gpu
 
 
-def compare(got, ref, tag):
-    for gi, (r, w) in enumerate(zip(got, ref)):
-        assert r.dp_cells == w["cells"], f"{tag} group {gi}: DP cells {r.dp_cells} != {w['cells']}"
-        for i in range(len(w["score"])):
-            if w["hash"][i] is None:
-                continue
-            assert r.read_best_score[i] == w["score"][i], f"{tag} group {gi} read {i}: score"
-            assert r.read_n_cigar[i] == w["n_cigar"][i], f"{tag} group {gi} read {i}: n_cigar"
-            assert int(r.read_cigar_hash[i]) == w["hash"][i], f"{tag} group {gi} read {i}: CIGAR hash"
-        assert len(r.cons) == len(w["cons"]) and all(np.array_equal(x, y) for x, y in zip(r.cons, w["cons"])), f"{tag} group {gi}: consensus"
-        assert all(np.array_equal(x, y) for x, y in zip(r.cov, w["cov"])), f"{tag} group {gi}: coverage"
-
-
 @pytest.mark.parametrize("engine", ["chain", "launch"])
 @pytest.mark.parametrize("name,n_groups", [("convex_10k", 4), ("affine_1k", 6), ("local_linear_5k", 1), ("aa_blosum62_2k", 2)])
-def test_full_shape(reference_lib, name, n_groups, engine):
-    """engine: the device-resident chain (default for global/banded/consensus runs) or the launch-per-round engine."""
+def test_full_shape(reference, name, n_groups, engine):
+    """engine: the engine's own choice, which is the device-resident chain for global/banded/consensus runs (local mode
+    always takes the launch engine, and must not touch the chain), or the launch-per-round engine forced."""
     w = synth.WORKLOADS[name]
-    if engine == "chain" and w.cfg.align_mode != 0:
-        pytest.skip("local mode always takes the launch engine")
     groups = w.groups(n_groups, base_seed=4200)
-    ref = reference_records(w.cfg, groups)
+    ref = reference.batch(w.cfg, groups)
     with BatchEngine() as eng:
         got = eng.run(w.cfg, groups, record_reads=True, no_chain=(engine == "launch"))
         st = eng.stats()
     if engine == "chain":
-        assert st["chain_groups"] == n_groups and st["chain_fallback_groups"] == 0, st
-    compare(got, ref, f"{name}/{engine}")
+        on_chain = n_groups if w.cfg.align_mode == 0 else 0
+        assert st["chain_groups"] == on_chain and st["chain_fallback_groups"] == 0, st
+    assert_batch_matches(got, groups, ref, f"{name}/{engine}", msa=False)
 
 
-def test_full_shape_convex_generic_kernels(reference_lib, monkeypatch):
+def test_full_shape_convex_generic_kernels(reference, monkeypatch):
     """The same 10 kbp x 50 shape with the packed kernel switched off: generic int16 planes while the reference's
     criterion allows (gn <= 16 364), int32 planes beyond -- both instantiations at full size."""
     monkeypatch.setenv("ABPOA_GPU_NO_P16", "1")
     w = synth.WORKLOADS["convex_10k"]
     groups = w.groups(1, base_seed=4300)
-    ref = reference_records(w.cfg, groups)
+    ref = reference.batch(w.cfg, groups)
     with BatchEngine(n_workers=1, groups_per_launch=1) as eng:
         got = eng.run(w.cfg, groups, record_reads=True)
-    compare(got, ref, "convex_10k/generic")
+    assert_batch_matches(got, groups, ref, "convex_10k/generic", msa=False)
