@@ -31,6 +31,8 @@ extern "C" cudaError_t poa_launch_align(int gap_mode, int bits, int align_mode, 
 extern "C" cudaError_t poa_launch_align_p16(int gap_mode, int align_mode, int lean, const int *gaps, const PoaJobDesc *jobs,
                                             const PoaParamsDev *prm, int n_jobs, int ring_rows, int ring_cells, cudaStream_t st);
 extern "C" void poa_pick_ring(int gap_mode, int bits, int band_cells, size_t smem_budget, int *ring_rows, int *ring_cells);
+extern "C" int poa_tma_enabled(void);
+extern "C" int poa_lean_disabled(void);
 
 #define CK(call) do { cudaError_t e_ = (call); if (e_ != cudaSuccess) \
     poa_die("libabpoa_b200/cuda", "%s failed at %s:%d: %s", #call, __FILE__, __LINE__, cudaGetErrorString(e_)); } while (0)
@@ -132,6 +134,7 @@ struct poa_dev_ctx {
     poa_capture_fn capture; void *capture_user;
     poa_pressure_fn pressure; void *pressure_user;   /* called before this context WAITS for plane memory */
     PoaJobDesc last_desc; int last_bits, last_gap, last_rows;   /* debug: job 0 of the most recent launch */
+    int last_lean, last_tma, last_ring_rows, last_ring_cells; uint64_t last_units;   /* ... how it ran, and its plane units used */
 };
 
 static void require_gpu(void) {
@@ -149,6 +152,7 @@ poa_dev_ctx *poa_dev_ctx_new_on(int dev) {
     c->h_in_cap = c->h_out_cap = c->d_in_cap = c->d_work_cap = c->d_planes_cap = c->h_res_cap = c->planes_limit = 0;
     memset(&c->stats, 0, sizeof c->stats); c->capture = NULL; c->capture_user = NULL; c->pressure = NULL; c->pressure_user = NULL; memset(&c->last_desc, 0, sizeof c->last_desc);
     c->last_bits = c->last_gap = c->last_rows = 0;
+    c->last_lean = c->last_tma = c->last_ring_rows = c->last_ring_cells = 0; c->last_units = 0;
     if (dev >= 0) { c->dev = dev; CK(cudaSetDevice(c->dev)); }
     else CK(cudaGetDevice(&c->dev));
     CK(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
@@ -362,6 +366,9 @@ static bool run_begin(poa_dev_ctx *c, const abpoa_para_t *abpt, poa_job *jobs, c
     int lean = !abpt->inc_path_score && abpt->align_mode == ABPOA_GLOBAL_MODE;
     for (int t = 0; t < n && lean; ++t) if (!jobs[idx[t]].plan.whole_graph) lean = 0;
     const int gaps[4] = { abpt->gap_ext1, abpt->gap_open1 + abpt->gap_ext1, abpt->gap_ext2, abpt->gap_open2 + abpt->gap_ext2 };
+    /* what poa_launch_align_p16 will instantiate (the TMA variant exists only with LEAN) */
+    c->last_lean = bits == 15 && lean && !poa_lean_disabled(); c->last_tma = c->last_lean && poa_tma_enabled();
+    c->last_ring_rows = ring_rows; c->last_ring_cells = ring_cells;
     if (bits == 15) CK(poa_launch_align_p16(abpt->gap_mode, abpt->align_mode, lean, gaps, (const PoaJobDesc *)(c->d_in + off_desc),
                                             (const PoaParamsDev *)c->d_in, n, ring_rows, ring_cells, c->st));
     else CK(poa_launch_align(abpt->gap_mode, bits, abpt->align_mode, (const PoaJobDesc *)(c->d_in + off_desc),
@@ -412,6 +419,7 @@ static void run_finish(poa_dev_ctx *c) {
 
     std::vector<PoaResultDev> resv(n);
     memcpy(resv.data(), c->h_res + 256, (size_t)n * sizeof(PoaResultDev));
+    c->last_units = resv[0].plane_units_used;
     std::vector<size_t> out_cig(n), out_band(n);
     for (int t = 0; t < n; ++t) {
         const poa_job &j = jobs[idx[t]];
@@ -648,6 +656,39 @@ extern "C" int poa_debug_fetch_row(abpoa_t *ab, int row, int32_t *out, int cap, 
             out[(size_t)p * cap + (j - ri.beg)] = S == 2 ? (int32_t)((int16_t *)buf.data())[k] : ((int32_t *)buf.data())[k];
         }
     return P;
+}
+
+/* debugging aid: the whole DP state of the most recent single alignment of `ab` in one copy each -- per row
+ * (beg, end, left, right) into rowinfo[4 * n_rows], the row's plane offset (8-cell units) into rowoff[n_rows], and the
+ * plane slab as the kernel stored it (int16 or int32 cells; a row's planes lie one after the other, each
+ * ((end >> 3) - (beg >> 3) + 1) * 8 cells wide -- except the generic kernel's banded linear-gap rows outside local mode
+ * ("lgx"), which are stored in whole reference vectors of pn = 16 / 8 cells, beg / pn * pn .. (end / pn + 1) * pn - 1)
+ * into `planes`.  Returns the slab's size in bytes (with planes == NULL or
+ * a `cap` that is too small: nothing is copied), or -1.  Rows the alignment never computed hold stale values. */
+extern "C" int64_t poa_debug_fetch_planes(abpoa_t *ab, int32_t *rowinfo, uint32_t *rowoff, void *planes, int64_t cap) {
+    poa_dev_ctx *c = (poa_dev_ctx *)ab->abm->s_mem;
+    if (!c || c->arena || c->last_rows <= 0) return -1;
+    const int64_t bytes = (int64_t)c->last_units * POA_GROUP * (c->last_bits == 32 ? 4 : 2);
+    if (!planes || cap < bytes) return bytes;
+    CK(cudaSetDevice(c->dev));
+    std::vector<PoaRowOff> ro(c->last_rows);
+    CK(cudaMemcpy(rowinfo, c->last_desc.rowinfo, (size_t)c->last_rows * sizeof(PoaRowInfo), cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(ro.data(), c->last_desc.rowoff, (size_t)c->last_rows * sizeof(PoaRowOff), cudaMemcpyDeviceToHost));
+    for (int r = 0; r < c->last_rows; ++r) rowoff[r] = ro[r].off;
+    if (bytes > 0) CK(cudaMemcpy(planes, c->last_desc.planes, (size_t)bytes, cudaMemcpyDeviceToHost));
+    return bytes;
+}
+
+/* debugging aid: how the most recent single alignment of `ab` ran, as it was finally accepted (after any redo):
+ * out[0] kernel (15 packed int16x2, 16 generic with int16 planes, 32 generic with int32 planes), out[1] LEAN predecessor
+ * path, out[2] TMA row staging, out[3] ring rows, out[4] ring cells, out[5] DP rows, out[6] planes per row,
+ * out[7] redo launches of the context so far.  Returns 0, or -1 before the first alignment. */
+extern "C" int poa_debug_last_run(abpoa_t *ab, int32_t *out8) {
+    poa_dev_ctx *c = (poa_dev_ctx *)ab->abm->s_mem;
+    if (!c || c->last_rows <= 0) return -1;
+    out8[0] = c->last_bits; out8[1] = c->last_lean; out8[2] = c->last_tma; out8[3] = c->last_ring_rows; out8[4] = c->last_ring_cells;
+    out8[5] = c->last_rows; out8[6] = planes_of(c->last_gap); out8[7] = (int32_t)c->stats.retries;
+    return 0;
 }
 
 /* debugging aid: redo launches (PLANE_OVF / RANGE) of the handle's single-alignment context so far */

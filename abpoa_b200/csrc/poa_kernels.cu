@@ -1776,6 +1776,8 @@ static cudaError_t launch_mode(int mode, const PoaJobDesc *jobs, const PoaParams
 /* Pick the shared-memory ring geometry for a launch: slots wide enough for the expected band
  * (`band_cells`, already a multiple of 8) and as many rows as fit the per-CTA budget. */
 extern "C" int poa_tma_enabled(void) { static const int on = [] { const char *e = getenv("ABPOA_GPU_TMA"); return e && *e == '1'; }(); return on; }
+/* ABPOA_GPU_NO_LEAN=1: whole-graph global jobs of the packed kernel take the general predecessor loop too */
+extern "C" int poa_lean_disabled(void) { static const int off = [] { const char *e = getenv("ABPOA_GPU_NO_LEAN"); return e && *e == '1'; }(); return off; }
 extern "C" void poa_pick_ring(int gap_mode, int bits, int band_cells, size_t smem_budget, int *ring_rows, int *ring_cells) {
     int rc = band_cells < 64 ? 64 : band_cells;
     int rr = 64;
@@ -1815,8 +1817,7 @@ extern "C" cudaError_t poa_launch_align_p16(int gap_mode, int align_mode, int le
                                             const PoaParamsDev *prm, int n_jobs, int ring_rows, int ring_cells, cudaStream_t st) {
     if (n_jobs <= 0) return cudaSuccess;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    static const int no_lean = [] { const char *e = getenv("ABPOA_GPU_NO_LEAN"); return e && *e == '1'; }();
-    if (no_lean) lean = 0;
+    if (poa_lean_disabled()) lean = 0;
     if (gap_mode == LG) return launch_p16_mode<LG>(align_mode, lean, jobs, prm, n_jobs, ring_rows, ring_cells, kc, st);
     if (gap_mode == AG) return launch_p16_mode<AG>(align_mode, lean, jobs, prm, n_jobs, ring_rows, ring_cells, kc, st);
     return launch_p16_mode<CG>(align_mode, lean, jobs, prm, n_jobs, ring_rows, ring_cells, kc, st);

@@ -1,78 +1,29 @@
 #!/usr/bin/env python
-"""Debug aid (GPU box): align with the product, then compare every DP row's planes and band
-with the scalar oracle, printing the first mismatching cell.
-usage: python tests/debug_planes.py <case-name> [read_index]"""
-import ctypes as C
+"""Debug aid (GPU box): align a named case of tests/cases.py with the product and compare every DP row's band, arg-max and
+planes with the scalar oracle after every read (tests/planes.py, the rule tests/test_gpu_planes.py asserts), printing
+which kernel ran and the first mismatching cells.
+usage: python tests/debug_planes.py <case-name>"""
 import sys
 from pathlib import Path
 
-import numpy as np
-
 ROOT = Path(__file__).resolve().parent.parent
 sys.path.insert(0, str(ROOT)); sys.path.insert(0, str(ROOT / "tests"))
-from abpoa_b200 import capi  # noqa: E402
-from abpoa_b200.aligner import PoaConfig, PoaSession  # noqa: E402
+from abpoa_b200.aligner import PoaConfig  # noqa: E402
 from cases import CASES, case_reads  # noqa: E402
-from oracle_binding import oracle_align  # noqa: E402
-
-NEG_LIMIT = -30000
+from planes import run_planes  # noqa: E402
 
 
 def main():
     name = sys.argv[1]
-    stop_at = int(sys.argv[2]) if len(sys.argv) > 2 else None
     case = CASES[name]
-    cfg = PoaConfig(**case["cfg"])
-    reads = case_reads(case)
-    lib = capi.product()
-    lib.dll.poa_debug_fetch_row.restype = C.c_int
-    lib.dll.poa_debug_fetch_row.argtypes = [capi.abpoa_t_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]
-    gpu = PoaSession(cfg, lib)
-    cpu = PoaSession(cfg, lib)          # host graph only; alignments from the oracle
-    gpu.reset(1024); cpu.reset(1024)
-    for ri, r in enumerate(reads):
-        rows = {}
 
-        def cb(user, row, beg, end, h, e1, e2, f1, f2):
-            wd = end - beg + 1
-            rows[row] = (beg, end, [np.ctypeslib.as_array(p, shape=(wd,)).copy() if p else None for p in (h, e1, e2, f1, f2)])
-        o, ores = oracle_align(cpu, r, row_cb=cb)
-        a, res = gpu.align(r)
-        if a.aligned:
-            print(f"read {ri}: gpu score {a.best_score} oracle {o.best_score} cigar_equal {np.array_equal(a.cigar, o.cigar)} cells {a.cells}/{o.cells}")
-            bad = 0
-            cap = len(r) + 16
-            buf = np.zeros((5, cap), dtype=np.int32)
-            info = np.zeros(4, dtype=np.int32)
-            for row in sorted(rows):
-                beg, end, pl = rows[row]
-                npl = lib.dll.poa_debug_fetch_row(gpu.ab, row, buf.ctypes.data, cap, info.ctypes.data)
-                if (info[0], info[1]) != (beg, end):
-                    print(f"  row {row}: band gpu ({info[0]},{info[1]}) oracle ({beg},{end})"); bad += 1; break
-                order = [0, 1, 3] if npl == 3 else ([0] if npl == 1 else [0, 1, 2, 3, 4])
-                for k, pi in enumerate(order):
-                    want = pl[pi]
-                    got = buf[k, : end - beg + 1]
-                    real = want > NEG_LIMIT * 1000
-                    diff = np.nonzero(real & (got != want))[0]
-                    if pi >= 3:   # F planes: first cell differs by construction
-                        diff = diff[diff > 0]
-                    if len(diff):
-                        j = diff[0]
-                        print(f"  row {row} plane {pi} j={beg + j}: gpu {got[j]} oracle {want[j]}  (band {beg}-{end}, {len(diff)} cells differ)")
-                        for kk, pp in enumerate(order):
-                            print(f"    plane {pp}: gpu {buf[kk, :12].tolist()} ... {buf[kk, end - beg - 5:end - beg + 1].tolist()}")
-                            print(f"    plane {pp}: ora {pl[pp][:12].tolist()} ... {pl[pp][-6:].tolist()}")
-                        bad += 1
-                        break
-                if bad:
-                    break
-            if not bad:
-                print("  all rows equal")
-            if bad or (stop_at is not None and ri >= stop_at):
-                break
-        cpu.add(r, ores, len(reads))
-        gpu.add(r, res, len(reads))
+    def show(i, info):
+        print(f"read {i}: {info.name} kernel, lean={int(info.lean)} tma={int(info.tma)} ring {info.ring_rows}x{info.ring_cells}: all rows equal")
+    try:
+        run_planes(PoaConfig(**case["cfg"]), case_reads(case), tag=name, check=show)
+    except AssertionError as e:
+        print(e)
+        sys.exit(1)
 
 
 if __name__ == "__main__":

@@ -28,6 +28,14 @@ def read_fasta(path: Path, m: int = 5) -> list[np.ndarray]:
     return seqs
 
 
+def deletion_fan(seed=7, n=40, flank=220):
+    """Reads that delete 1..n-1 bases in front of the same template position: that node collects one
+    in-edge per read (> 32 predecessors: the chunked predecessor loops of the DP and of the backtrace)."""
+    rng = np.random.default_rng(seed)
+    t = rng.integers(0, 4, size=2 * flank).astype(np.uint8)
+    return [t] + [np.concatenate([t[: flank - k], t[flank:]]) for k in range(1, n)]
+
+
 def run_group(lib, cfg: PoaConfig, reads, want_msa: bool = True, use_oracle: bool = False, fast_order: bool = False, weights=None):
     """Progressive POA of one group through `lib`; returns per-read records + consensus (+ MSA).
 

@@ -35,8 +35,8 @@ def oracle():
     return _dll
 
 
-def oracle_align(session, codes: np.ndarray, want_bands: bool = False, row_cb=None):
-    """Align `codes` to the graph owned by `session` with the scalar oracle.
+def oracle_align(session, codes: np.ndarray, want_bands: bool = False, row_cb=None, beg_node_id: int = 0, end_node_id: int = 1):
+    """Align `codes` to the graph owned by `session` (or to its sub-graph between two node ids) with the scalar oracle.
     Returns (ReadAlignment, abpoa_res_t[, beg, end])."""
     codes = np.ascontiguousarray(codes, dtype=np.uint8)
     g = session.ab.contents.abg.contents
@@ -56,7 +56,7 @@ def oracle_align(session, codes: np.ndarray, want_bands: bool = False, row_cb=No
         info.dp_beg = beg.ctypes.data_as(c_int_p)
         info.dp_end = end.ctypes.data_as(c_int_p)
         info.band_cap = g.node_n
-    oracle().poa_oracle_align_sequence_to_subgraph(session.ab, session.abpt, 0, 1, codes.ctypes.data_as(c_u8_p), len(codes),
+    oracle().poa_oracle_align_sequence_to_subgraph(session.ab, session.abpt, beg_node_id, end_node_id, codes.ctypes.data_as(c_u8_p), len(codes),
                                                    C.byref(res), C.byref(info))
     cig = np.ctypeslib.as_array(res.graph_cigar, shape=(res.n_cigar,)).copy() if res.n_cigar > 0 else np.zeros(0, dtype=np.uint64)
     out = ReadAlignment(True, int(res.best_score), cig, res.node_s, res.node_e, res.query_s, res.query_e, int(info.cells), info.n_rows - 1)

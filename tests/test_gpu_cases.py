@@ -23,7 +23,7 @@ from abpoa_b200.aligner import PoaConfig, PoaSession
 from abpoa_b200.batch import BatchEngine, fnv1a_words
 from abpoa_b200.capi import abpoa_res_t, c_u8_p
 from cases import AFFINE, CASES, case_reads, case_weights
-from helpers import assert_digest_equal, group_digest, run_group
+from helpers import assert_digest_equal, deletion_fan, group_digest, run_group
 from reference_runs import Hasher, assert_batch_matches, assert_run_matches
 
 pytestmark = pytest.mark.gpu
@@ -146,14 +146,6 @@ def test_batch_no_p16_and_slab_redo(reference, monkeypatch):
 
 
 # ------------------------------------------------------------------------------------------- graph shapes
-def deletion_fan(seed=7, n=40, flank=220):
-    """Reads that delete 1..n-1 bases in front of the same template position: that node collects one
-    in-edge per read (> 32 predecessors: the chunked predecessor loops of the DP and of the backtrace)."""
-    rng = np.random.default_rng(seed)
-    t = rng.integers(0, 4, size=2 * flank).astype(np.uint8)
-    return [t] + [np.concatenate([t[: flank - k], t[flank:]]) for k in range(1, n)]
-
-
 def max_in_degree(lib, cfg, reads):
     with PoaSession(cfg, lib) as s:
         s.run_reads(reads, count_cells=False)
