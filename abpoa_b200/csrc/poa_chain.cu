@@ -223,7 +223,9 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
     const int m = abpt->m;
     const int K = [&] { const char *e = getenv("ABPOA_GPU_CHAIN_K"); return e && *e ? atoi(e) : (m > 5 ? 24 : 12); }();
     const int A = m - 1 > 1 ? m - 1 : 1;
-    const int P = abpt->gap_mode == ABPOA_LINEAR_GAP ? 1 : (abpt->gap_mode == ABPOA_AFFINE_GAP ? 3 : 5);
+    /* plane units (16 B) per 8-cell group of a DP row, times 2: the chain's kernels store H (+E1 (+E2)) and one byte of
+     * insertion decisions per cell (RowLayout in poa_kernels.cu) */
+    const int P2 = abpt->gap_mode == ABPOA_LINEAR_GAP ? 2 : (abpt->gap_mode == ABPOA_AFFINE_GAP ? 5 : 7);
     int n_cohorts = [&] { const char *e = getenv("ABPOA_GPU_CHAIN_COHORTS"); return e && *e ? atoi(e) : 4; }();
     if (n_cohorts < 1) n_cohorts = 1;
     if (n_cohorts > 16) n_cohorts = 16;
@@ -268,7 +270,10 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
             if (ok && !poa_p16_ok(abpt, l, 3 * l)) ok = false;
         }
         if (!ok || p.qmax > (1 << 24)) { fallback.push_back(g); continue; }
-        const int64_t grow = (int64_t)((double)p.qmax * (1.0 + 0.10 * (p.n_reads - 1))) + 256;
+        /* node capacity: 10 % growth per read, and for large groups at most 4 % plus a fixed slack (5 % error, 50 x 10 kbp:
+         * 3.0 % measured, 33.8k nodes reserved for 25k used) -- a group that outgrows it goes to the launch engine */
+        const int64_t grow = std::min<int64_t>((int64_t)((double)p.qmax * (1.0 + 0.10 * (p.n_reads - 1))) + 256,
+                                               (int64_t)((double)p.qmax * (1.0 + 0.04 * (p.n_reads - 1))) + 4096);
         p.n_cap = (int)std::min<int64_t>(2 + p.bases, grow);
         const size_t nc = (size_t)p.n_cap, scr_n = std::max<size_t>((size_t)p.qmax + 2, nc);
         size_t b = 0;
@@ -287,9 +292,15 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         b += al256(sizeof(PoaResultDev)) + al256(nc * sizeof(PoaBtRec));
         if (record) b += 2 * al256((size_t)p.n_reads * 4) + al256((size_t)p.n_reads * 8);
         p.static_bytes = b;
+        /* plane units of the group's largest (last) alignment.  Free-running, a group's slab is private and its rows take
+         * what their bands really need: rows 3.2 % growth per read, 2w+1 cells plus the 8-cell grid per row (5 % error,
+         * 50 x 10 kbp: 25.0k rows, 29-30.4 groups per row measured; estimate 25.8k x 30).  The round schedule bump-allocates
+         * every job's band ESTIMATE (chain_flatten: +64 cells, + length drift) from a shared pool: keep the roomier figures. */
         const int wmax = poa_band_halfwidth(abpt, p.qmax);
-        const double rows_final = std::min<double>(2.0 + (double)p.bases, (double)p.qmax * (1.0 + 0.045 * (p.n_reads - 1)) + 64);
-        p.pool_units_est = rows_final * (double)((2 * wmax + 1 + 32 + 7) / 8 + 2) * P;
+        const double growth = free_run ? 0.032 : 0.045;
+        const int band_slack = free_run ? 0 : 32;
+        const double rows_final = std::min<double>(2.0 + (double)p.bases, (double)p.qmax * (1.0 + growth * (p.n_reads - 1)) + 64);
+        p.pool_units_est = rows_final * (double)((2 * wmax + 1 + band_slack + 7) / 8 + 2) * P2 / 2;
         plans.push_back(p);
     }
     if (plans.empty()) return 0;
@@ -462,7 +473,7 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         }
         PoaChainParams hcp; memset(&hcp, 0, sizeof hcp);
         hcp.K = K; hcp.A = A; hcp.m = m; hcp.max_mat = abpt->max_mat; hcp.min_mis = abpt->min_mis; hcp.o1 = abpt->gap_open1; hcp.e1 = abpt->gap_ext1;
-        hcp.oe1 = abpt->gap_open1 + abpt->gap_ext1; hcp.oe2 = abpt->gap_open2 + abpt->gap_ext2; hcp.record = record ? 1 : 0; hcp.P = P;
+        hcp.oe1 = abpt->gap_open1 + abpt->gap_ext1; hcp.oe2 = abpt->gap_open2 + abpt->gap_ext2; hcp.record = record ? 1 : 0; hcp.P2 = P2;
         PoaParamsDev hprm; poa_fill_params(&hprm, abpt, 15);
 
         /* ---- upload (stream 0 of the wave), then fork the cohort streams ---- */

@@ -60,7 +60,8 @@ typedef struct PoaChainParams {         /* one per batch call */
     int32_t K, A;                       /* inline edge slots per node and direction / aligned-set slots */
     int32_t m, max_mat, min_mis, o1, e1, oe1, oe2;      /* for the reference's score-width rule (pn) */
     int32_t record;                     /* keep per-read score / CIGAR length / FNV-1a hash */
-    int32_t P;                          /* score planes per DP row (1 / 3 / 5)              */
+    int32_t P2;                         /* plane units per 8-cell group of a DP row, times 2 (compact
+                                           layout: H, E planes + one byte per cell; 2 / 5 / 7) */
 } PoaChainParams;
 
 typedef struct PoaChainSlot {           /* one per read group; every pointer aims into the group's HBM region */
@@ -314,7 +315,7 @@ POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int3
             unsigned long long per_row = (unsigned long long)((2 * w + 1 + drift + 64 + 7) / 8 + 2);
             const unsigned long long full = (unsigned long long)((qlen + 1 + 7) / 8 + 1);
             if (generous || per_row > full) per_row = full;
-            const unsigned long long units = per_row * (unsigned long long)cp->P * (unsigned long long)n;
+            const unsigned long long units = (per_row * (unsigned long long)cp->P2 + 1) / 2 * (unsigned long long)n;
             if (!s->pool_cursor) {                                     /* private slab: the job may use all of it */
                 s->jd.planes = s->pool_base; s->jd.plane_cap_units = s->pool_units;
             } else {

@@ -97,6 +97,20 @@ template <int GAP> struct Planes {
     static constexpr int H = 0, E1 = 1, E2 = 2, F1 = (GAP == AG ? 2 : 3), F2 = 4;
 };
 
+/* Compact row layout (FB, the chain engine's packed kernel): H (+E1 (+E2)) as int16 planes, then instead of the F planes
+ * one byte per cell holding the outcome of every comparison the backtrace's insertion step makes on them.  For F plane k
+ * (bits 3k..3k+2):
+ *   FB_A  H[i][j] == F_k[i][j]
+ *   FB_B  H[i][j-1] - oe_k == F_k[i][j]     (0 when j-1 is outside the band)
+ *   FB_C  F_k[i][j-1] - e_k == F_k[i][j]    (0 when j-1 is outside the band)
+ * Cells outside the band are 0.  A row of ngrp 8-cell groups takes ngrp * N16 + ceil(ngrp / 2) 16-byte units. */
+enum { FB_A = 1, FB_B = 2, FB_C = 4 };
+template <int GAP, bool FB> struct RowLayout {
+    static constexpr int N16 = FB ? (GAP == LG ? 1 : (GAP == AG ? 2 : 3)) : Planes<GAP>::N;   /* int16 planes in HBM */
+    static constexpr bool BITS = FB && GAP != LG;                                              /* linear gaps need no F */
+    __host__ __device__ static constexpr uint32_t units(uint32_t ngrp) { return ngrp * N16 + (BITS ? (ngrp + 1) / 2 : 0); }
+};
+
 /* Blob loads: plain coherent loads (blobs may be produced on the device by an earlier kernel of the
  * same stream; nothing here relies on the read-only path). */
 template <typename T> __device__ __forceinline__ T ldb(const T *p) { return *p; }
@@ -143,6 +157,11 @@ template <typename ST> struct BtRow {
         pstride = (g1 - g0 + 1) * POA_GROUP;
         ptr = planes + ((ptrdiff_t)off - g0) * POA_GROUP;
     }
+    /* compact layout: &bits[row][0] (virtual, like ptr), the byte plane behind the n16 int16 planes */
+    __device__ __forceinline__ const uint8_t *fbits(int n16) const {
+        const int c0 = (beg >> 3) << 3;
+        return reinterpret_cast<const uint8_t *>(ptr + c0 + n16 * pstride) - c0;
+    }
 };
 template <typename ST>
 __device__ __forceinline__ void bt_load_row(BtRow<ST> &r, const JobView &jv, const ST *planes, const PoaRowInfo *rowinfo, const PoaRowOff *rowoff, int row, int xs = 3) {
@@ -173,10 +192,11 @@ struct CigarSink {
     __device__ __forceinline__ void del(int node_id) { flush(); emit(((uint64_t)node_id << 34) | (1ull << 4) | 2u); }
 };
 
-template <int GAP, typename ST, int MODE>
+template <int GAP, typename ST, int MODE, bool FB = false>
 __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const PoaParamsDev *prm, const int *mat_s,
                               int lane, int best_i, int best_j, PoaResultDev &res, int xs = 3, const PoaBtRec *btrec = nullptr) {
     typedef Planes<GAP> PL;
+    typedef RowLayout<GAP, FB> RL;
     const ST *planes = reinterpret_cast<const ST *>(jd.planes);
     const PoaRowInfo *rowinfo = jd.rowinfo; const PoaRowOff *rowoff = jd.rowoff;
     const int m = prm->m, e1 = prm->e1, oe1 = prm->oe1, e2 = prm->e2, oe2 = prm->oe2;
@@ -296,7 +316,8 @@ __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const Poa
                         const ST *cell = planes + (size_t)r_off * POA_GROUP + kb;
                         const size_t gplane = (size_t)r_ngrp * POA_GROUP;
 #pragma unroll
-                        for (int pl = 0; pl < PL::N; ++pl) asm volatile("prefetch.global.L1 [%0];" :: "l"(cell + pl * gplane));
+                        for (int pl = 0; pl < RL::N16; ++pl) asm volatile("prefetch.global.L1 [%0];" :: "l"(cell + pl * gplane));
+                        if (RL::BITS) asm volatile("prefetch.global.L1 [%0];" :: "l"(reinterpret_cast<const uint8_t *>(cell - kb + RL::N16 * gplane) + kb));
                     }
                 }
                 if (r == 0) break;
@@ -357,7 +378,8 @@ __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const Poa
                 asm volatile("prefetch.global.L1 [%0];" :: "l"(pc.ptr + PL::E1 * pc.pstride + j));
                 if (GAP == CG) asm volatile("prefetch.global.L1 [%0];" :: "l"(pc.ptr + PL::E2 * pc.pstride + j));
             }
-            if (lane < PL::N && me.has(j)) asm volatile("prefetch.global.L1 [%0];" :: "l"(me.ptr + lane * me.pstride + j));
+            if (lane < RL::N16 && me.has(j)) asm volatile("prefetch.global.L1 [%0];" :: "l"(me.ptr + lane * me.pstride + j));
+            if (RL::BITS && lane == RL::N16 && me.has(j)) asm volatile("prefetch.global.L1 [%0];" :: "l"(me.fbits(RL::N16) + j));
         }
         const bool c_in_m = pc.has(j - 1);
         const int c_hm1 = c_in_m ? (int)pc.ptr[j - 1] : NEG;
@@ -453,6 +475,20 @@ __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const Poa
             const int h_jm1 = in_jm1 ? (int)me.ptr[j - 1] : NEG;
             if (GAP == LG) {
                 if (h_jm1 - e1 == h_ij) hit = 1;
+            } else if (RL::BITS) {                                      /* the comparisons below, made by the forward pass */
+                const int fb = in_j ? (int)me.fbits(RL::N16)[j] : 0;
+                if (GAP == AG || (cur & OP_F1)) {
+                    if (!(cur & OP_M) || (fb & FB_A)) {
+                        if (fb & FB_B) { cur = OP_M | OP_E; hit = 1; }
+                        else if (fb & FB_C) { cur = OP_F1; hit = 1; }
+                    }
+                }
+                if (GAP == CG && !hit && (cur & OP_F2)) {
+                    if (!(cur & OP_M) || (fb & (FB_A << 3))) {
+                        if (fb & (FB_B << 3)) { cur = OP_M | OP_E; hit = 1; }
+                        else if (fb & (FB_C << 3)) { cur = OP_F2; hit = 1; }
+                    }
+                }
             } else {
                 if (GAP == AG || (cur & OP_F1)) {
                     const int f_ij = in_j ? (int)me.ptr[PL::F1 * me.pstride + j] : NEG;
@@ -1011,11 +1047,14 @@ __device__ __forceinline__ P16Smem p16_smem_init(uint8_t *dyn_smem, const PoaPar
  * bulk-copy engine (cp.async.bulk shared -> global, one copy per plane, issued by one lane) instead of five 16-byte
  * stores per lane; a slot is reused ring_rows rows later, after cp.async.bulk.wait_group.read says the engine has
  * finished reading it.  Rows wider than a ring slot keep the plain stores. */
-template <int GAP, int MODE, bool LEAN = false, bool TMA = false>
+/* FB: the compact row layout (RowLayout): the F planes are replaced by one byte of backtrace decisions per cell. */
+template <int GAP, int MODE, bool LEAN = false, bool TMA = false, bool FB = false>
 __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParamsDev *__restrict__ prm, const P16Consts &kc, const P16Smem &sm,
                                             int ring_rows, int ring_cells, int lane) {
+    static_assert(!(TMA && FB), "the TMA row drain stages the five-plane layout");
     typedef int16_t ST;
     typedef Planes<GAP> PL;
+    typedef RowLayout<GAP, FB> RL;
     constexpr int RN = RingPlanes<GAP>::N;
     int *mat_s = sm.mat_s; uint4 *cap_lo = sm.cap_lo, *cap_hi = sm.cap_hi, *ring_meta = sm.ring_meta; ST *ring_data = sm.ring_data;
     const int rmask = ring_rows - 1, ring_groups = ring_cells >> 3;
@@ -1055,7 +1094,7 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
         int end0 = qlen;
         if (banded) end0 = min(qlen, max(0, qlen - jv.remain(0)) + w);
         const int g1 = end0 >> 3, ngrp = g1 + 1;
-        if ((uint64_t)ngrp * PL::N > jd.plane_cap_units) { if (lane == 0) { res.status = POA_ST_PLANE_OVF; *jd.result = res; } return; }
+        if ((uint64_t)RL::units(ngrp) > jd.plane_cap_units) { if (lane == 0) { res.status = POA_ST_PLANE_OVF; *jd.result = res; } return; }
         for (int gp = 0; gp <= g1; gp += 32) {
             const int g = gp + lane;
             if (g <= g1) {
@@ -1074,8 +1113,12 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
                 }
                 ST *rp = planes + (size_t)g * POA_GROUP;
                 st8(rp, h);
-                if (GAP != LG) { st8(rp + (size_t)PL::E1 * ngrp * POA_GROUP, ea); st8(rp + (size_t)PL::F1 * ngrp * POA_GROUP, fa); }
-                if (GAP == CG) { st8(rp + (size_t)PL::E2 * ngrp * POA_GROUP, eb); st8(rp + (size_t)PL::F2 * ngrp * POA_GROUP, fb); }
+                if (GAP != LG) st8(rp + (size_t)PL::E1 * ngrp * POA_GROUP, ea);
+                if (GAP == CG) st8(rp + (size_t)PL::E2 * ngrp * POA_GROUP, eb);
+                if (!FB && GAP != LG) st8(rp + (size_t)PL::F1 * ngrp * POA_GROUP, fa);
+                if (!FB && GAP == CG) st8(rp + (size_t)PL::F2 * ngrp * POA_GROUP, fb);
+                if (RL::BITS)                                /* the backtrace never takes a step in row 0 */
+                    *reinterpret_cast<uint2 *>(reinterpret_cast<uint8_t *>(planes + (size_t)RL::N16 * ngrp * POA_GROUP) + (size_t)g * 8) = make_uint2(0u, 0u);
                 if (g < ring_groups) {
                     ST *rq = ring_data + (size_t)g * POA_GROUP;
                     st8(rq, h);
@@ -1088,7 +1131,7 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
             PoaRowInfo r0; r0.beg = 0; r0.end = end0; r0.left = 0; r0.right = 0;
             rowinfo[0] = r0; { PoaRowOff z; z.off = 0; z.p0 = -1; rowoff[0] = z; } ring_meta[0] = make_uint4(0u, (unsigned)end0, 1u | (1u << 16), 0u);
         }
-        cursor = (uint64_t)ngrp * PL::N;
+        cursor = RL::units(ngrp);
         cells += end0 + 1; max_band = end0 + 1;
         __syncwarp();
     }
@@ -1203,7 +1246,7 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
             if (np > 0 && (beg >> pn_shift) < (min_pre_beg >> pn_shift)) beg = min_pre_beg;   /* reference's vector-granular clamp */
         }
         const int g0 = beg >> 3, g1 = end >> 3, ngrp = g1 - g0 + 1;
-        const uint32_t need = (uint32_t)ngrp * PL::N;
+        const uint32_t need = RL::units((uint32_t)ngrp);
         if (need > cap32 - cur32) {
             if (TMA) { if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); __syncwarp(); }     /* nothing may still read this CTA's smem */
             if (lane == 0) { res.status = POA_ST_PLANE_OVF; res.plane_units_used = cur32; *jd.result = res; }
@@ -1230,6 +1273,7 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
         }
 
         int carry1 = 2 * NEG, carry2 = 2 * NEG;
+        unsigned fb_h = 0u, fb_f1 = 0u, fb_f2 = 0u;           /* FB: H / F cells left of lane 0 on the next pass (high halves) */
         int row_max = NEG, row_left = -1, row_right = -1;
         KP(0)
 
@@ -1446,6 +1490,39 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
                     *reinterpret_cast<uint4 *>(rec) = make_uint4((unsigned)(g0 * 8), (unsigned)mypred,
                                                                  (unsigned)rbase | (ngrp <= POA_BTREC_GROUPS ? 0x100u : 0u) | ((unsigned)min(ngrp, 0xffff) << 16), (unsigned)my_off);
             }
+            /* FB: the insertion-step comparisons of the backtrace on the values stored for this row (exact: every value is
+             * >= NEGP and every penalty <= 1000 (poa_p16_ok), so the packed additions cannot wrap) */
+            uint2 fbits = make_uint2(0u, 0u);
+            if (RL::BITS) {
+                const unsigned hl = __shfl_up_sync(FULL, H[3], 1), f1l = __shfl_up_sync(FULL, F1[3], 1);
+                unsigned f2l = 0u;
+                if (GAP == CG) f2l = __shfl_up_sync(FULL, F2[3], 1);
+                const unsigned hp = lane == 0 ? fb_h : hl, f1p = lane == 0 ? fb_f1 : f1l, f2p = lane == 0 ? fb_f2 : f2l;
+                /* cell 8g-1 is inside the band exactly when g > g0 (beg lies in group g0) */
+                const unsigned clp = g > g0 ? 0x7fff0000u : 0u;
+                unsigned v[4];
+#pragma unroll
+                for (int k = 0; k < 4; ++k) {
+                    const unsigned inb = __vcmpeq2(CAP[k], 0x7fff7fffu);                          /* j in the band   */
+                    const unsigned inl = inb & __vcmpeq2(sh1(k ? CLO[k - 1] : clp, CLO[k]), 0x7fff7fffu);   /* and j-1 too */
+                    const unsigned hs = sh1(k ? H[k - 1] : hp, H[k]), fs1 = sh1(k ? F1[k - 1] : f1p, F1[k]);
+                    unsigned x = (__vcmpeq2(H[k], F1[k]) & inb & (FB_A * 0x10001u))
+                               | (__vcmpeq2(__vadd2(hs, kc.NOE1), F1[k]) & inl & (FB_B * 0x10001u))
+                               | (__vcmpeq2(__vadd2(fs1, kc.NE1), F1[k]) & inl & (FB_C * 0x10001u));
+                    if (GAP == CG) {
+                        const unsigned fs2 = sh1(k ? F2[k - 1] : f2p, F2[k]);
+                        x |= (__vcmpeq2(H[k], F2[k]) & inb & ((FB_A << 3) * 0x10001u))
+                           | (__vcmpeq2(__vadd2(hs, kc.NOE2), F2[k]) & inl & ((FB_B << 3) * 0x10001u))
+                           | (__vcmpeq2(__vadd2(fs2, kc.NE2), F2[k]) & inl & ((FB_C << 3) * 0x10001u));
+                    }
+                    v[k] = x;
+                }
+                fbits = make_uint2(__byte_perm(v[0], v[1], 0x6420), __byte_perm(v[2], v[3], 0x6420));
+                if (g1 - gp >= 32) {                            /* uniform: another pass follows */
+                    fb_h = __shfl_sync(FULL, H[3], 31); fb_f1 = __shfl_sync(FULL, F1[3], 31);
+                    if (GAP == CG) fb_f2 = __shfl_sync(FULL, F2[3], 31);
+                }
+            }
             KP(2)
             if (TMA && tma_row) {
                 if (gp == g0) {                              /* the slot's previous tenant (ring_rows rows ago) must have been read out */
@@ -1475,14 +1552,11 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
                 }
                 ST *q = rowp + (size_t)rel * POA_GROUP;
                 *reinterpret_cast<uint4 *>(q) = make_uint4(H[0], H[1], H[2], H[3]);
-                if (GAP != LG) {
-                    *reinterpret_cast<uint4 *>(q + (size_t)PL::E1 * gplane) = make_uint4(E1o[0], E1o[1], E1o[2], E1o[3]);
-                    *reinterpret_cast<uint4 *>(q + (size_t)PL::F1 * gplane) = make_uint4(F1[0], F1[1], F1[2], F1[3]);
-                }
-                if (GAP == CG) {
-                    *reinterpret_cast<uint4 *>(q + (size_t)PL::E2 * gplane) = make_uint4(E2o[0], E2o[1], E2o[2], E2o[3]);
-                    *reinterpret_cast<uint4 *>(q + (size_t)PL::F2 * gplane) = make_uint4(F2[0], F2[1], F2[2], F2[3]);
-                }
+                if (GAP != LG) *reinterpret_cast<uint4 *>(q + (size_t)PL::E1 * gplane) = make_uint4(E1o[0], E1o[1], E1o[2], E1o[3]);
+                if (GAP == CG) *reinterpret_cast<uint4 *>(q + (size_t)PL::E2 * gplane) = make_uint4(E2o[0], E2o[1], E2o[2], E2o[3]);
+                if (!FB && GAP != LG) *reinterpret_cast<uint4 *>(q + (size_t)PL::F1 * gplane) = make_uint4(F1[0], F1[1], F1[2], F1[3]);
+                if (!FB && GAP == CG) *reinterpret_cast<uint4 *>(q + (size_t)PL::F2 * gplane) = make_uint4(F2[0], F2[1], F2[2], F2[3]);
+                if (RL::BITS) *reinterpret_cast<uint2 *>(reinterpret_cast<uint8_t *>(rowp + (size_t)RL::N16 * gplane) + (size_t)rel * 8) = fbits;
             }
 
             KP(3)
@@ -1577,7 +1651,7 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
     if (lane == 0) *jd.result = res;
     __syncwarp();
     if (prm->ret_cigar && res.status == POA_ST_OK) {
-        poa_backtrack<GAP, ST, MODE>(jv, jd, prm, mat_s, lane, best_i, best_j, *jd.result, 3, jd.btrec);
+        poa_backtrack<GAP, ST, MODE, FB>(jv, jd, prm, mat_s, lane, best_i, best_j, *jd.result, 3, jd.btrec);
         if (lane == 0) jd.result->bt_clk = clock64() - clk1;
     }
 }
@@ -1609,7 +1683,7 @@ static inline size_t ring_smem_bytes(int gap, int bits, int ring_rows, int ring_
  * The same job function, fed from device-resident slots (poa_chain.cuh): the job blob of a slot is written
  * by the fuse kernel of the previous round, nothing comes from the host.  Block 0 also zeroes the plane-pool
  * cursor the coming fuse kernel will fill (see PoaChainSlot). */
-template <int GAP, bool TMA>
+template <int GAP>
 __global__ void POA_P16_BOUNDS poa_chain_align_kernel_p16(const PoaChainSlot *__restrict__ slots, const int32_t *__restrict__ idx,
                                                            const PoaParamsDev *__restrict__ prm, int n_jobs, int round, int ring_rows, int ring_cells,
                                                            const __grid_constant__ P16Consts kc) {
@@ -1623,7 +1697,7 @@ __global__ void POA_P16_BOUNDS poa_chain_align_kernel_p16(const PoaChainSlot *__
     const int n_rows = reinterpret_cast<const PoaJobHeader *>(jd.blob)->n_rows;
     if (sl->failed || sl->fused >= sl->n_reads || n_rows < 3) { if (lane == 0) jd.result->status = POA_ST_SKIP; return; }
     const P16Smem sm = p16_smem_init(dyn_smem, prm, ring_rows, lane);
-    p16_run_job<GAP, GLOBAL, true, TMA>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
+    p16_run_job<GAP, GLOBAL, true, false, true>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
 }
 
 /* Free-running chain (PoaChainSync in poa_chain.cuh): one resident warp per group runs the group's alignments back to
@@ -1633,7 +1707,7 @@ __device__ __forceinline__ int chain_ld_relaxed(const int32_t *p) { int v; asm v
 __device__ __forceinline__ void chain_st_relaxed(int32_t *p, int v) { asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ unsigned long long chain_now_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
-template <int GAP, bool TMA>
+template <int GAP>
 __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, PoaChainSync *sync, const PoaParamsDev *__restrict__ prm, int n_groups,
                                                           int ring_rows, int ring_cells, int dbg, const __grid_constant__ P16Consts kc) {
     extern __shared__ __align__(16) uint8_t dyn_smem[];
@@ -1672,7 +1746,7 @@ __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, P
         const PoaJobDesc jd = sl->jd;
         const int n_rows = reinterpret_cast<const PoaJobHeader *>(jd.blob)->n_rows;
         if (sl->failed || sl->fused >= sl->n_reads || n_rows < 3) break;
-        p16_run_job<GAP, GLOBAL, true, TMA>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
+        p16_run_job<GAP, GLOBAL, true, false, true>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
         __syncwarp();
         if (!(dbg & 1)) __threadfence();                       /* release side: CIGAR + result are out before the task is */
         if (lane == 0) {
@@ -1691,58 +1765,50 @@ __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, P
     }
 }
 
-template <int GAP, bool TMA>
+template <int GAP>
 static cudaError_t launch_chain_worker_one(PoaChainSlot *slots, PoaChainSync *sync, int n_groups, const PoaParamsDev *prm, int ring_rows, int ring_cells,
                                            const P16Consts &kc, cudaStream_t st) {
     /* at least 23 KB: at most 9 of these CTAs fit one SM, which leaves registers (9 x 160 x 32 of 64 K) and shared memory for a
      * 256-thread fuse worker next to them even if the alignment warps were dispatched first -- they wait for fuse workers */
     /* experiment hooks (timing only): ABPOA_GPU_CHAIN_DBG bit 0 = no fences (UNSAFE), bit 1 = no shared-memory padding; ABPOA_GPU_CHAIN_CARVEOUT */
     static const int dbg = [] { const char *e = getenv("ABPOA_GPU_CHAIN_DBG"); return e && *e ? atoi(e) : 0; }();
-    const size_t smem0 = ring_smem_bytes(GAP, 16, ring_rows, ring_cells, TMA) + 18 * sizeof(uint4);
+    const size_t smem0 = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
     const size_t smem = (dbg & 2) ? smem0 : std::max<size_t>(smem0, (size_t)23 * 1024);
-    cudaError_t e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return e;
     /* the same L1/shared split as the fuse workers ask for (poa_chain.cu): CTAs of both kernels share SMs for the whole run */
     { const char *cv = getenv("ABPOA_GPU_CHAIN_CARVEOUT");
-      e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, TMA>, cudaFuncAttributePreferredSharedMemoryCarveout, cv && *cv ? atoi(cv) : (int)cudaSharedmemCarveoutMaxShared);
+      e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP>, cudaFuncAttributePreferredSharedMemoryCarveout, cv && *cv ? atoi(cv) : (int)cudaSharedmemCarveoutMaxShared);
       if (e != cudaSuccess) return e; }
-    poa_chain_dp_worker_kernel<GAP, TMA><<<n_groups, 32, smem, st>>>(slots, sync, prm, n_groups, ring_rows, ring_cells, dbg, kc);
+    poa_chain_dp_worker_kernel<GAP><<<n_groups, 32, smem, st>>>(slots, sync, prm, n_groups, ring_rows, ring_cells, dbg, kc);
     return cudaGetLastError();
 }
-extern "C" int poa_tma_enabled(void);
 extern "C" cudaError_t poa_launch_chain_dp_worker(int gap_mode, const int *gaps, PoaChainSlot *slots, PoaChainSync *sync, int n_groups,
                                                   const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st) {
     if (n_groups <= 0) return cudaSuccess;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    const bool tma = poa_tma_enabled() && ring_rows >= 2;
-    if (gap_mode == LG) return tma ? launch_chain_worker_one<LG, true>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st) : launch_chain_worker_one<LG, false>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st);
-    if (gap_mode == AG) return tma ? launch_chain_worker_one<AG, true>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st) : launch_chain_worker_one<AG, false>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st);
-    return tma ? launch_chain_worker_one<CG, true>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st) : launch_chain_worker_one<CG, false>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == LG) return launch_chain_worker_one<LG>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == AG) return launch_chain_worker_one<AG>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st);
+    return launch_chain_worker_one<CG>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st);
 }
 
-template <int GAP, bool TMA>
+template <int GAP>
 static cudaError_t launch_chain_one(const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round, const PoaParamsDev *prm, int ring_rows, int ring_cells,
                                     const P16Consts &kc, cudaStream_t st) {
-    const size_t smem = ring_smem_bytes(GAP, 16, ring_rows, ring_cells, TMA) + 18 * sizeof(uint4);
-    cudaError_t e = cudaFuncSetAttribute(poa_chain_align_kernel_p16<GAP, TMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    const size_t smem = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_align_kernel_p16<GAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return e;
-    poa_chain_align_kernel_p16<GAP, TMA><<<n_jobs, 32, smem, st>>>(slots, idx, prm, n_jobs, round, ring_rows, ring_cells, kc);
+    poa_chain_align_kernel_p16<GAP><<<n_jobs, 32, smem, st>>>(slots, idx, prm, n_jobs, round, ring_rows, ring_cells, kc);
     return cudaGetLastError();
 }
 /* gaps[4] = { e1, oe1, e2, oe2 } (host copy of what prm holds on the device) */
-extern "C" int poa_tma_enabled(void);
 extern "C" cudaError_t poa_launch_chain_align_p16(int gap_mode, const int *gaps, const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round,
                                                   const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st) {
     if (n_jobs <= 0) return cudaSuccess;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    if (poa_tma_enabled() && ring_rows >= 2) {
-        if (gap_mode == LG) return launch_chain_one<LG, true>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
-        if (gap_mode == AG) return launch_chain_one<AG, true>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
-        return launch_chain_one<CG, true>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
-    }
-    if (gap_mode == LG) return launch_chain_one<LG, false>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
-    if (gap_mode == AG) return launch_chain_one<AG, false>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
-    return launch_chain_one<CG, false>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == LG) return launch_chain_one<LG>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == AG) return launch_chain_one<AG>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
+    return launch_chain_one<CG>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
 }
 
 /* ------------------------------------------------------------------ launcher */
