@@ -223,9 +223,9 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
     const int m = abpt->m;
     const int K = [&] { const char *e = getenv("ABPOA_GPU_CHAIN_K"); return e && *e ? atoi(e) : (m > 5 ? 24 : 12); }();
     const int A = m - 1 > 1 ? m - 1 : 1;
-    /* plane units (16 B) per 8-cell group of a DP row, times 2: the chain's kernels store H (+E1 (+E2)) and one byte of
-     * insertion decisions per cell (RowLayout in poa_kernels.cu) */
-    const int P2 = abpt->gap_mode == ABPOA_LINEAR_GAP ? 2 : (abpt->gap_mode == ABPOA_AFFINE_GAP ? 5 : 7);
+    /* plane units (16 B) per 8-cell group of a DP row: the chain's kernels store H (+E1 (+E2)) and no F planes (RowLayout in
+     * poa_kernels.cu) */
+    const int P = abpt->gap_mode == ABPOA_LINEAR_GAP ? 1 : (abpt->gap_mode == ABPOA_AFFINE_GAP ? 2 : 3);
     int n_cohorts = [&] { const char *e = getenv("ABPOA_GPU_CHAIN_COHORTS"); return e && *e ? atoi(e) : 4; }();
     if (n_cohorts < 1) n_cohorts = 1;
     if (n_cohorts > 16) n_cohorts = 16;
@@ -300,7 +300,7 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         const double growth = free_run ? 0.032 : 0.045;
         const int band_slack = free_run ? 0 : 32;
         const double rows_final = std::min<double>(2.0 + (double)p.bases, (double)p.qmax * (1.0 + growth * (p.n_reads - 1)) + 64);
-        p.pool_units_est = rows_final * (double)((2 * wmax + 1 + band_slack + 7) / 8 + 2) * P2 / 2;
+        p.pool_units_est = rows_final * (double)((2 * wmax + 1 + band_slack + 7) / 8 + 2) * P;
         plans.push_back(p);
     }
     if (plans.empty()) return 0;
@@ -473,7 +473,7 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         }
         PoaChainParams hcp; memset(&hcp, 0, sizeof hcp);
         hcp.K = K; hcp.A = A; hcp.m = m; hcp.max_mat = abpt->max_mat; hcp.min_mis = abpt->min_mis; hcp.o1 = abpt->gap_open1; hcp.e1 = abpt->gap_ext1;
-        hcp.oe1 = abpt->gap_open1 + abpt->gap_ext1; hcp.oe2 = abpt->gap_open2 + abpt->gap_ext2; hcp.record = record ? 1 : 0; hcp.P2 = P2;
+        hcp.oe1 = abpt->gap_open1 + abpt->gap_ext1; hcp.oe2 = abpt->gap_open2 + abpt->gap_ext2; hcp.record = record ? 1 : 0; hcp.P = P;
         PoaParamsDev hprm; poa_fill_params(&hprm, abpt, 15);
 
         /* ---- upload (stream 0 of the wave), then fork the cohort streams ---- */
@@ -705,9 +705,10 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         if (verbose) {
             double pf[6] = {0, 0, 0, 0, 0, 0}; double na = 0;
             for (int t = 0; t < nw; ++t) { for (int z = 0; z < 6; ++z) pf[z] += (double)fin[t].prof[z]; na += fin[t].fused > 0 ? fin[t].fused - 1 : 0; }
-            double bd[4] = {0, 0, 0, 0};
-            for (int t = 0; t < nw; ++t) for (int z = 0; z < 4; ++z) bd[z] += (double)fin[t].btdiag[z];
-            if (na > 0) fprintf(stderr, "[chain, backtrace per alignment] %.0f steps in %.0f speculative rounds, %.0f general steps costing %.0f k-cycles\n", bd[0] / na, bd[1] / na, bd[2] / na, bd[3] / na);
+            double bd[5] = {0, 0, 0, 0, 0};
+            for (int t = 0; t < nw; ++t) for (int z = 0; z < 5; ++z) bd[z] += (double)fin[t].btdiag[z];
+            if (na > 0) fprintf(stderr, "[chain, backtrace per alignment] %.0f steps in %.0f speculative rounds, %.0f general steps costing %.0f k-cycles, "
+                                        "%.1f rows with their F planes recomputed\n", bd[0] / na, bd[1] / na, bd[2] / na, bd[3] / na, bd[4] / na);
             if (na > 0) fprintf(stderr, "[chain, k-cycles/alignment] -DPOA_KPROF phases: setup %.0f pred %.0f compute %.0f store %.0f rowmax %.0f tail+prefetch %.0f\n",
                                 pf[0] / na / 1e3, pf[1] / na / 1e3, pf[2] / na / 1e3, pf[3] / na / 1e3, pf[4] / na / 1e3, pf[5] / na / 1e3);
         }

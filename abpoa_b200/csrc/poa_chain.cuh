@@ -60,8 +60,8 @@ typedef struct PoaChainParams {         /* one per batch call */
     int32_t K, A;                       /* inline edge slots per node and direction / aligned-set slots */
     int32_t m, max_mat, min_mis, o1, e1, oe1, oe2;      /* for the reference's score-width rule (pn) */
     int32_t record;                     /* keep per-read score / CIGAR length / FNV-1a hash */
-    int32_t P2;                         /* plane units per 8-cell group of a DP row, times 2 (compact
-                                           layout: H, E planes + one byte per cell; 2 / 5 / 7) */
+    int32_t P;                          /* plane units per 8-cell group of a DP row (compact layout:
+                                           H and the E planes; 1 / 2 / 3) */
 } PoaChainParams;
 
 typedef struct PoaChainSlot {           /* one per read group; every pointer aims into the group's HBM region */
@@ -96,7 +96,7 @@ typedef struct PoaChainSlot {           /* one per read group; every pointer aim
     int32_t rsv0;
     unsigned long long wait_ns, fuse_ns;        /* time the alignment warp waited for its fuse tasks / time inside chain_fuse */
     int64_t prof[6];                    /* -DPOA_KPROF builds: per-phase cycles of the forward row loop, summed over the alignments */
-    int64_t btdiag[4];                  /* -DPOA_KPROF builds: PoaResultDev.btdiag summed */
+    int64_t btdiag[5];                  /* -DPOA_KPROF builds: PoaResultDev.btdiag summed */
     /* per-read records (record mode) */
     int32_t *rec_score, *rec_nops; uint64_t *rec_hash;
 } PoaChainSlot;
@@ -315,7 +315,7 @@ POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int3
             unsigned long long per_row = (unsigned long long)((2 * w + 1 + drift + 64 + 7) / 8 + 2);
             const unsigned long long full = (unsigned long long)((qlen + 1 + 7) / 8 + 1);
             if (generous || per_row > full) per_row = full;
-            const unsigned long long units = (per_row * (unsigned long long)cp->P2 + 1) / 2 * (unsigned long long)n;
+            const unsigned long long units = per_row * (unsigned long long)cp->P * (unsigned long long)n;
             if (!s->pool_cursor) {                                     /* private slab: the job may use all of it */
                 s->jd.planes = s->pool_base; s->jd.plane_cap_units = s->pool_units;
             } else {
@@ -407,7 +407,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
         s->cells += res->cells; s->fwd_clk += res->fwd_clk; s->bt_clk += res->bt_clk;
 #ifdef POA_KPROF
         for (int z = 0; z < 6; ++z) s->prof[z] += res->prof[z];
-        for (int z = 0; z < 4; ++z) s->btdiag[z] += res->btdiag[z];
+        for (int z = 0; z < 5; ++z) s->btdiag[z] += res->btdiag[z];
 #endif
         if (cp->record) {
             s->rec_score[r] = res->best_score; s->rec_nops[r] = n_ops;

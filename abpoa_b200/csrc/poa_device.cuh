@@ -57,8 +57,8 @@ typedef struct PoaResultDev {
     int64_t prof[6];                    /* optional per-phase SM cycles (ABPOA kernel built with -DPOA_KPROF) */
     int32_t diag[4];                    /* -DPOA_KPROF: rows on the straight-line path / rows sent to the generic path because of
                                            > 2 predecessors / a predecessor outside the ring / a predecessor band wider than its ring slot */
-    int32_t btdiag[4];                  /* -DPOA_KPROF: backtrace steps taken by the speculative shortcut / its rounds / general steps /
-                                           k-cycles spent in general steps */
+    int32_t btdiag[5];                  /* -DPOA_KPROF: backtrace steps taken by the speculative shortcut / its rounds / general steps /
+                                           k-cycles spent in general steps / rows whose F planes the insertion step recomputed */
 } PoaResultDev;
 
 /* Backtrace shortcut record of one DP row, written by the packed forward kernel (64 B, one cache-line half):

@@ -97,18 +97,19 @@ template <int GAP> struct Planes {
     static constexpr int H = 0, E1 = 1, E2 = 2, F1 = (GAP == AG ? 2 : 3), F2 = 4;
 };
 
-/* Compact row layout (FB, the chain engine's packed kernel): H (+E1 (+E2)) as int16 planes, then instead of the F planes
- * one byte per cell holding the outcome of every comparison the backtrace's insertion step makes on them.  For F plane k
+/* Compact row layout (FB, the chain engine's packed kernel): only H (+E1 (+E2)) as int16 planes, no F planes.  The F
+ * planes are read by nothing but the backtrace's insertion step, which recomputes them for the one row it needs them in
+ * (fb_recompute) and keeps, per cell, one byte with the outcome of every comparison it makes on them.  For F plane k
  * (bits 3k..3k+2):
  *   FB_A  H[i][j] == F_k[i][j]
  *   FB_B  H[i][j-1] - oe_k == F_k[i][j]     (0 when j-1 is outside the band)
  *   FB_C  F_k[i][j-1] - e_k == F_k[i][j]    (0 when j-1 is outside the band)
- * Cells outside the band are 0.  A row of ngrp 8-cell groups takes ngrp * N16 + ceil(ngrp / 2) 16-byte units. */
+ * Cells outside the band are 0.  A row of ngrp 8-cell groups takes ngrp * N16 16-byte units. */
 enum { FB_A = 1, FB_B = 2, FB_C = 4 };
 template <int GAP, bool FB> struct RowLayout {
     static constexpr int N16 = FB ? (GAP == LG ? 1 : (GAP == AG ? 2 : 3)) : Planes<GAP>::N;   /* int16 planes in HBM */
     static constexpr bool BITS = FB && GAP != LG;                                              /* linear gaps need no F */
-    __host__ __device__ static constexpr uint32_t units(uint32_t ngrp) { return ngrp * N16 + (BITS ? (ngrp + 1) / 2 : 0); }
+    __host__ __device__ static constexpr uint32_t units(uint32_t ngrp) { return ngrp * N16; }
 };
 
 /* Blob loads: plain coherent loads (blobs may be produced on the device by an earlier kernel of the
@@ -157,11 +158,6 @@ template <typename ST> struct BtRow {
         pstride = (g1 - g0 + 1) * POA_GROUP;
         ptr = planes + ((ptrdiff_t)off - g0) * POA_GROUP;
     }
-    /* compact layout: &bits[row][0] (virtual, like ptr), the byte plane behind the n16 int16 planes */
-    __device__ __forceinline__ const uint8_t *fbits(int n16) const {
-        const int c0 = (beg >> 3) << 3;
-        return reinterpret_cast<const uint8_t *>(ptr + c0 + n16 * pstride) - c0;
-    }
 };
 template <typename ST>
 __device__ __forceinline__ void bt_load_row(BtRow<ST> &r, const JobView &jv, const ST *planes, const PoaRowInfo *rowinfo, const PoaRowOff *rowoff, int row, int xs = 3) {
@@ -192,9 +188,20 @@ struct CigarSink {
     __device__ __forceinline__ void del(int node_id) { flush(); emit(((uint64_t)node_id << 34) | (1ull << 4) | 2u); }
 };
 
+/* What the backtrace of the compact layout needs to recompute a row's F planes (fb_recompute, after the packed kernel) */
+struct P16Consts;
+struct FbCtx {
+    const P16Consts *kc; const uint4 *cap_lo, *cap_hi;   /* the packed kernel's constants and band-mask tables          */
+    uint8_t *buf; int buf_cells;                          /* decision bytes of one row: the shared-memory ring, idle now */
+};
+template <int GAP, int MODE>
+__device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaParamsDev *prm, const FbCtx &fx,
+                            int beg, int end, int pb, int np, int base, int j, int lane);
+
 template <int GAP, typename ST, int MODE, bool FB = false>
 __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const PoaParamsDev *prm, const int *mat_s,
-                              int lane, int best_i, int best_j, PoaResultDev &res, int xs = 3, const PoaBtRec *btrec = nullptr) {
+                              int lane, int best_i, int best_j, PoaResultDev &res, int xs = 3, const PoaBtRec *btrec = nullptr,
+                              const FbCtx *fx = nullptr) {
     typedef Planes<GAP> PL;
     typedef RowLayout<GAP, FB> RL;
     const ST *planes = reinterpret_cast<const ST *>(jd.planes);
@@ -205,8 +212,9 @@ __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const Poa
     CigarSink cg; cg.out = jd.cigar; cg.cap = jd.cigar_cap; cg.n = 0; cg.pending = 0; cg.lane = lane; cg.ovf = 0;
 
     int i = best_i, j = best_j, start_i = best_i, start_j = best_j, cur = OP_ALL;
+    int fb_row = -1, fb_lo = 0;                 /* FB: fx->buf holds the decision bytes of row fb_row from cell fb_lo on */
 #ifdef POA_KPROF
-    int bd_steps = 0, bd_rounds = 0, bd_general = 0; long long bd_clk = 0;
+    int bd_steps = 0, bd_rounds = 0, bd_general = 0, bd_fbrows = 0; long long bd_clk = 0;
 #endif
     int n_aln = 0, n_match = 0, err = 0;
     int gap_at_end = prm->put_gap_at_end; const int gap_on_right = prm->put_gap_on_right;
@@ -317,7 +325,6 @@ __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const Poa
                         const size_t gplane = (size_t)r_ngrp * POA_GROUP;
 #pragma unroll
                         for (int pl = 0; pl < RL::N16; ++pl) asm volatile("prefetch.global.L1 [%0];" :: "l"(cell + pl * gplane));
-                        if (RL::BITS) asm volatile("prefetch.global.L1 [%0];" :: "l"(reinterpret_cast<const uint8_t *>(cell - kb + RL::N16 * gplane) + kb));
                     }
                 }
                 if (r == 0) break;
@@ -379,7 +386,6 @@ __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const Poa
                 if (GAP == CG) asm volatile("prefetch.global.L1 [%0];" :: "l"(pc.ptr + PL::E2 * pc.pstride + j));
             }
             if (lane < RL::N16 && me.has(j)) asm volatile("prefetch.global.L1 [%0];" :: "l"(me.ptr + lane * me.pstride + j));
-            if (RL::BITS && lane == RL::N16 && me.has(j)) asm volatile("prefetch.global.L1 [%0];" :: "l"(me.fbits(RL::N16) + j));
         }
         const bool c_in_m = pc.has(j - 1);
         const int c_hm1 = c_in_m ? (int)pc.ptr[j - 1] : NEG;
@@ -475,8 +481,15 @@ __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const Poa
             const int h_jm1 = in_jm1 ? (int)me.ptr[j - 1] : NEG;
             if (GAP == LG) {
                 if (h_jm1 - e1 == h_ij) hit = 1;
-            } else if (RL::BITS) {                                      /* the comparisons below, made by the forward pass */
-                const int fb = in_j ? (int)me.fbits(RL::N16)[j] : 0;
+            } else if constexpr (RL::BITS) {                            /* the comparisons below, on the recomputed F planes */
+                if (in_j && (i != fb_row || j < fb_lo)) {               /* first insertion step of this row (or left of the window) */
+                    fb_lo = fb_recompute<GAP, MODE>(jv, jd, prm, *fx, me.beg, me.end, me.pb, me.np, me.base, j, lane);
+                    fb_row = i;
+#ifdef POA_KPROF
+                    ++bd_fbrows;
+#endif
+                }
+                const int fb = in_j ? (int)fx->buf[j - fb_lo] : 0;
                 if (GAP == AG || (cur & OP_F1)) {
                     if (!(cur & OP_M) || (fb & FB_A)) {
                         if (fb & FB_B) { cur = OP_M | OP_E; hit = 1; }
@@ -523,7 +536,7 @@ __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const Poa
         res.n_aln_bases = n_aln; res.n_matched_bases = n_match;
         if (err) res.status = POA_ST_BT_ERROR; else if (cg.ovf) res.status = POA_ST_CIGAR_OVF;
 #ifdef POA_KPROF
-        res.btdiag[0] = bd_steps; res.btdiag[1] = bd_rounds; res.btdiag[2] = bd_general; res.btdiag[3] = (int)(bd_clk >> 10);
+        res.btdiag[0] = bd_steps; res.btdiag[1] = bd_rounds; res.btdiag[2] = bd_general; res.btdiag[3] = (int)(bd_clk >> 10); res.btdiag[4] = bd_fbrows;
 #endif
     }
 }
@@ -1037,6 +1050,186 @@ __device__ __forceinline__ P16Smem p16_smem_init(uint8_t *dyn_smem, const PoaPar
     return sm;
 }
 
+/* The row arithmetic of one lane's 8 cells (group g, jr0 = 8 (g - g0)), shared by the forward pass and the backtrace's F
+ * recompute so that both give the same bits: from the folded predecessor terms (M: diagonal, X1 / X2: vertical), the query
+ * profile S and the band masks to H, the F planes and the outgoing E planes.  carry1 / carry2 carry the F scans from one
+ * 256-cell pass to the next; M is left holding Hm, -inf left of the band. */
+template <int GAP, int MODE>
+__device__ __forceinline__ void p16_cells(const P16Consts &kc, const unsigned CLO[4], const unsigned CAP[4], const unsigned S[4],
+                                          unsigned M[4], const unsigned X1[4], const unsigned X2[4], int jr0, int e1, int oe1, int e2, int oe2,
+                                          unsigned zr2, int lane, int &carry1, int &carry2,
+                                          unsigned H[4], unsigned F1[4], unsigned F2[4], unsigned E1o[4], unsigned E2o[4]) {
+    unsigned T[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const unsigned hm = __viaddmax_s16x2(M[k], S[k], NEGP2);
+        M[k] = __vmins2(hm, CLO[k]);                                 /* Hm, -inf left of the band */
+        if (GAP == LG) T[k] = __vmins2(__vmaxs2(hm, X1[k]), CLO[k]);
+        else if (GAP == AG) T[k] = M[k];                              /* affine F opens from the M-only value */
+        else T[k] = __vmins2(__vimax3_s16x2(hm, X1[k], X2[k]), CLO[k]);
+    }
+    /* lane-local A = T + e*c ; lane aggregate in 32 bits ; warp scan ; back to lane-local */
+    unsigned a1[4], a2[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) { a1[k] = __vadd2(T[k], kc.K1[k]); if (GAP == CG) a2[k] = __vadd2(T[k], kc.K2[k]); }
+    const int off1 = e1 * jr0 - (GAP == LG ? 0 : oe1), off2 = e2 * jr0 - oe2;
+    int tot1, tot2 = 0;
+    int x1 = max(warp_excl_max(lane_max8(a1) + off1, lane, tot1), carry1);
+    carry1 = max(carry1, tot1);
+    const int xl1 = min(max(x1 - off1, NEGP), 32767);
+    unsigned P1[4], P2[4];
+    lane_excl_prefix(a1, pk(xl1, xl1), P1);
+    if (GAP == CG) {
+        int x2 = max(warp_excl_max(lane_max8(a2) + off2, lane, tot2), carry2);
+        carry2 = max(carry2, tot2);
+        const int xl2 = min(max(x2 - off2, NEGP), 32767);
+        lane_excl_prefix(a2, pk(xl2, xl2), P2);
+    }
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        if (GAP == LG) {
+            /* inclusive: H[c] = max(P[c], a[c]) - e1*c */
+            unsigned h = __viaddmax_s16x2(__vmaxs2(P1[k], a1[k]), kc.KLG[k], NEGP2);
+            if (MODE == LOCAL) h = __vmaxs2(h, zr2);
+            H[k] = __vmins2(h, CAP[k]);
+        } else {
+            F1[k] = __viaddmax_s16x2(P1[k], kc.KF1[k], NEGP2);
+            if (GAP == AG) {
+                const unsigned t = __vmaxs2(M[k], X1[k]);
+                unsigned fz = F1[k];
+                if (MODE == LOCAL) fz = __vmaxs2(fz, zr2);
+                const unsigned h = __vmaxs2(t, fz);
+                const unsigned from_t = __vcmpges2(t, fz);            /* h == t, per cell */
+                const unsigned ev = __viaddmax_s16x2(X1[k], kc.NE1, __viaddmax_s16x2(h, kc.NOE1, NEGP2));
+                const unsigned alt = (MODE == LOCAL) ? zr2 : NEGP2;
+                E1o[k] = __vmins2((ev & from_t) | (alt & ~from_t), CAP[k]);
+                H[k] = __vmins2(h, CAP[k]);
+            } else {
+                F2[k] = __viaddmax_s16x2(P2[k], kc.KF2[k], NEGP2);
+                unsigned h = __vimax3_s16x2(T[k], F1[k], F2[k]);
+                if (MODE == LOCAL) h = __vmaxs2(h, zr2);
+                unsigned eo1 = __viaddmax_s16x2(X1[k], kc.NE1, __viaddmax_s16x2(h, kc.NOE1, NEGP2));
+                unsigned eo2 = __viaddmax_s16x2(X2[k], kc.NE2, __viaddmax_s16x2(h, kc.NOE2, NEGP2));
+                if (MODE == LOCAL) { eo1 = __vmaxs2(eo1, zr2); eo2 = __vmaxs2(eo2, zr2); }
+                H[k] = __vmins2(h, CAP[k]); E1o[k] = __vmins2(eo1, CAP[k]); E2o[k] = __vmins2(eo2, CAP[k]);
+            }
+        }
+    }
+}
+
+/* The insertion-step decision bytes (FB_A / FB_B / FB_C, see RowLayout) of one lane's 8 cells from the values p16_cells gave
+ * (exact: every value is >= NEGP and every penalty <= 1000 (poa_p16_ok), so the packed additions cannot wrap).  left_in:
+ * cell 8g-1 is inside the band (g > g0, as beg lies in group g0).  lh / lf1 / lf2 hold H / F of the cell left of lane 0 (high
+ * halves, from the previous pass); more: another pass follows, so they are set to lane 31's last cell. */
+template <int GAP>
+__device__ __forceinline__ uint2 p16_fbits(const P16Consts &kc, const unsigned H[4], const unsigned F1[4], const unsigned F2[4],
+                                           const unsigned CLO[4], const unsigned CAP[4], bool left_in, int lane, bool more,
+                                           unsigned &lh, unsigned &lf1, unsigned &lf2) {
+    const unsigned hl = __shfl_up_sync(FULL, H[3], 1), f1l = __shfl_up_sync(FULL, F1[3], 1);
+    unsigned f2l = 0u;
+    if (GAP == CG) f2l = __shfl_up_sync(FULL, F2[3], 1);
+    const unsigned hp = lane == 0 ? lh : hl, f1p = lane == 0 ? lf1 : f1l, f2p = lane == 0 ? lf2 : f2l;
+    const unsigned clp = left_in ? 0x7fff0000u : 0u;
+    unsigned v[4];
+#pragma unroll
+    for (int k = 0; k < 4; ++k) {
+        const unsigned inb = __vcmpeq2(CAP[k], 0x7fff7fffu);                          /* j in the band   */
+        const unsigned inl = inb & __vcmpeq2(sh1(k ? CLO[k - 1] : clp, CLO[k]), 0x7fff7fffu);   /* and j-1 too */
+        const unsigned hs = sh1(k ? H[k - 1] : hp, H[k]), fs1 = sh1(k ? F1[k - 1] : f1p, F1[k]);
+        unsigned x = (__vcmpeq2(H[k], F1[k]) & inb & (FB_A * 0x10001u))
+                   | (__vcmpeq2(__vadd2(hs, kc.NOE1), F1[k]) & inl & (FB_B * 0x10001u))
+                   | (__vcmpeq2(__vadd2(fs1, kc.NE1), F1[k]) & inl & (FB_C * 0x10001u));
+        if (GAP == CG) {
+            const unsigned fs2 = sh1(k ? F2[k - 1] : f2p, F2[k]);
+            x |= (__vcmpeq2(H[k], F2[k]) & inb & ((FB_A << 3) * 0x10001u))
+               | (__vcmpeq2(__vadd2(hs, kc.NOE2), F2[k]) & inl & ((FB_B << 3) * 0x10001u))
+               | (__vcmpeq2(__vadd2(fs2, kc.NE2), F2[k]) & inl & ((FB_C << 3) * 0x10001u));
+        }
+        v[k] = x;
+    }
+    if (more) {
+        lh = __shfl_sync(FULL, H[3], 31); lf1 = __shfl_sync(FULL, F1[3], 31);
+        if (GAP == CG) lf2 = __shfl_sync(FULL, F2[3], 31);
+    }
+    return make_uint2(__byte_perm(v[0], v[1], 0x6420), __byte_perm(v[2], v[3], 0x6420));
+}
+
+/* Recompute row `row`'s F planes for the backtrace's insertion step (compact layout): the row arithmetic of the forward pass
+ * (p16_cells), fed from the predecessors' H / E planes in HBM, the query profile and the band-mask tables, pass by pass from
+ * the band's first cell to cell j.  The decision bytes of the last fx.buf_cells / 256 passes up to j's go to fx.buf, from the
+ * returned cell on.  Jobs of the compact layout run the LEAN forward pass, which has no path scores (chain jobs carry none). */
+template <int GAP, int MODE>
+__device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaParamsDev *prm, const FbCtx &fx,
+                            int beg, int end, int pb, int np, int base, int j, int lane) {
+    const P16Consts &kc = *fx.kc;
+    const int16_t *planes = reinterpret_cast<const int16_t *>(jd.planes);
+    const int e1 = prm->e1, oe1 = prm->oe1, e2 = prm->e2, oe2 = prm->oe2;
+    const unsigned zr2 = (unsigned)prm->zero;
+    const int qstride = ((jv.qlen + 1 + 7) & ~7) + 8;
+    const int16_t *qrow = jd.qprof + (size_t)base * qstride;
+    const int g0 = beg >> 3, g1 = end >> 3;
+    const int pj = ((j >> 3) - g0) >> 5;                              /* j's pass */
+    const int p_lo = max(0, pj - max(fx.buf_cells >> 8, 1) + 1);      /* first pass kept in the buffer */
+    const int lo = (g0 + 32 * p_lo) * 8;
+    int carry1 = 2 * NEG, carry2 = 2 * NEG;
+    unsigned lh = 0u, lf1 = 0u, lf2 = 0u;
+    for (int p = 0; p <= pj; ++p) {
+        const int gp = g0 + 32 * p, g = gp + lane;
+        const bool active = g <= g1;
+        uint4 sv = make_uint4(0u, 0u, 0u, 0u);
+        if (active) sv = *reinterpret_cast<const uint4 *>(qrow + (size_t)g * 8);
+        unsigned M[4], X1[4], X2[4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) { M[k] = NEGP2; X1[k] = NEGP2; X2[k] = NEGP2; }
+        const bool fix_left = (gp > g0) || ((beg & 7) == 0);
+        for (int kb = 0; kb < np; kb += 32) {
+            int c_g0 = 0, c_ng = 0; uint32_t c_off = 0;                /* predecessor kb + lane: first group, groups, slab offset */
+            if (kb + lane < np) {
+                const int prow = ldb(jv.pred + pb + kb + lane);
+                const PoaRowInfo pi = jd.rowinfo[prow];
+                c_g0 = pi.beg >> 3; c_ng = (pi.end >> 3) - c_g0 + 1; c_off = jd.rowoff[prow].off;
+            }
+            const int nk = min(32, np - kb);
+            for (int k = 0; k < nk; ++k) {
+                const int pg0 = __shfl_sync(FULL, c_g0, k), png = __shfl_sync(FULL, c_ng, k);
+                const uint32_t off = __shfl_sync(FULL, c_off, k);
+                const int16_t *ph = planes + (size_t)off * POA_GROUP;
+                const size_t pp = (size_t)png * POA_GROUP;
+                const int rel = g - pg0;
+                uint4 hp = make_uint4(NEGP2, NEGP2, NEGP2, NEGP2), ep1 = hp, ep2 = hp;
+                if (active && (unsigned)rel < (unsigned)png) {
+                    const int16_t *q = ph + (size_t)rel * POA_GROUP;
+                    hp = *reinterpret_cast<const uint4 *>(q);
+                    if (GAP != LG) ep1 = *reinterpret_cast<const uint4 *>(q + (size_t)Planes<GAP>::E1 * pp);
+                    if (GAP == CG) ep2 = *reinterpret_cast<const uint4 *>(q + (size_t)Planes<GAP>::E2 * pp);
+                }
+                unsigned prev = __shfl_up_sync(FULL, hp.w, 1);
+                if (lane == 0) {
+                    int hm1 = NEGP;
+                    if (fix_left && (unsigned)(rel - 1) < (unsigned)png) hm1 = (int)ph[(size_t)(rel - 1) * POA_GROUP + 7];
+                    if (MODE == LOCAL && g == 0) hm1 = 0;
+                    prev = (unsigned)hm1 << 16;
+                }
+                M[0] = __vmaxs2(M[0], sh1(prev, hp.x)); M[1] = __vmaxs2(M[1], sh1(hp.x, hp.y));
+                M[2] = __vmaxs2(M[2], sh1(hp.y, hp.z)); M[3] = __vmaxs2(M[3], sh1(hp.z, hp.w));
+                X1[0] = __vmaxs2(X1[0], ep1.x); X1[1] = __vmaxs2(X1[1], ep1.y); X1[2] = __vmaxs2(X1[2], ep1.z); X1[3] = __vmaxs2(X1[3], ep1.w);
+                if (GAP == CG) { X2[0] = __vmaxs2(X2[0], ep2.x); X2[1] = __vmaxs2(X2[1], ep2.y); X2[2] = __vmaxs2(X2[2], ep2.z); X2[3] = __vmaxs2(X2[3], ep2.w); }
+            }
+        }
+        const int nlo = min(max(beg - g * 8, 0), 8), nhi = min(max(g * 8 + 7 - end, 0), 8);
+        const uint4 clo = fx.cap_lo[nlo], chi = fx.cap_hi[nhi];
+        const unsigned CLO[4] = { clo.x, clo.y, clo.z, clo.w };
+        const unsigned CAP[4] = { __vmins2(clo.x, chi.x), __vmins2(clo.y, chi.y), __vmins2(clo.z, chi.z), __vmins2(clo.w, chi.w) };
+        const unsigned S[4] = { sv.x, sv.y, sv.z, sv.w };
+        unsigned H[4], F1[4], F2[4], E1o[4], E2o[4];
+        p16_cells<GAP, MODE>(kc, CLO, CAP, S, M, X1, X2, (g - g0) * 8, e1, oe1, e2, oe2, zr2, lane, carry1, carry2, H, F1, F2, E1o, E2o);
+        const uint2 bits = p16_fbits<GAP>(kc, H, F1, F2, CLO, CAP, g > g0, lane, p < pj, lh, lf1, lf2);
+        if (p >= p_lo && active) *reinterpret_cast<uint2 *>(fx.buf + (g * 8 - lo)) = bits;
+    }
+    __syncwarp();
+    return lo;
+}
+
 /* One alignment job on one warp: forward DP + backtrace.  Writes *jd.result (every status) but does
  * NOT publish completion -- the caller does (signal_done), after whatever it still has to move. */
 /* LEAN (whole-graph jobs without -G path scores): rows with one or two predecessors that are still in the
@@ -1047,7 +1240,7 @@ __device__ __forceinline__ P16Smem p16_smem_init(uint8_t *dyn_smem, const PoaPar
  * bulk-copy engine (cp.async.bulk shared -> global, one copy per plane, issued by one lane) instead of five 16-byte
  * stores per lane; a slot is reused ring_rows rows later, after cp.async.bulk.wait_group.read says the engine has
  * finished reading it.  Rows wider than a ring slot keep the plain stores. */
-/* FB: the compact row layout (RowLayout): the F planes are replaced by one byte of backtrace decisions per cell. */
+/* FB: the compact row layout (RowLayout): no F planes; the backtrace recomputes them where it needs them (fb_recompute). */
 template <int GAP, int MODE, bool LEAN = false, bool TMA = false, bool FB = false>
 __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParamsDev *__restrict__ prm, const P16Consts &kc, const P16Smem &sm,
                                             int ring_rows, int ring_cells, int lane) {
@@ -1117,8 +1310,6 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
                 if (GAP == CG) st8(rp + (size_t)PL::E2 * ngrp * POA_GROUP, eb);
                 if (!FB && GAP != LG) st8(rp + (size_t)PL::F1 * ngrp * POA_GROUP, fa);
                 if (!FB && GAP == CG) st8(rp + (size_t)PL::F2 * ngrp * POA_GROUP, fb);
-                if (RL::BITS)                                /* the backtrace never takes a step in row 0 */
-                    *reinterpret_cast<uint2 *>(reinterpret_cast<uint8_t *>(planes + (size_t)RL::N16 * ngrp * POA_GROUP) + (size_t)g * 8) = make_uint2(0u, 0u);
                 if (g < ring_groups) {
                     ST *rq = ring_data + (size_t)g * POA_GROUP;
                     st8(rq, h);
@@ -1273,7 +1464,6 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
         }
 
         int carry1 = 2 * NEG, carry2 = 2 * NEG;
-        unsigned fb_h = 0u, fb_f1 = 0u, fb_f2 = 0u;           /* FB: H / F cells left of lane 0 on the next pass (high halves) */
         int row_max = NEG, row_left = -1, row_right = -1;
         KP(0)
 
@@ -1418,63 +1608,8 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
             const unsigned CAP[4] = { __vmins2(clo.x, chi.x), __vmins2(clo.y, chi.y), __vmins2(clo.z, chi.z), __vmins2(clo.w, chi.w) };
             const unsigned S[4] = { sv.x, sv.y, sv.z, sv.w };
 
-            unsigned T[4], H[4], F1[4], F2[4], E1o[4], E2o[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                const unsigned hm = __viaddmax_s16x2(M[k], S[k], NEGP2);
-                M[k] = __vmins2(hm, CLO[k]);                                 /* Hm, -inf left of the band */
-                if (GAP == LG) T[k] = __vmins2(__vmaxs2(hm, X1[k]), CLO[k]);
-                else if (GAP == AG) T[k] = M[k];                              /* affine F opens from the M-only value */
-                else T[k] = __vmins2(__vimax3_s16x2(hm, X1[k], X2[k]), CLO[k]);
-            }
-            /* lane-local A = T + e*c ; lane aggregate in 32 bits ; warp scan ; back to lane-local */
-            const int jr0 = (g - g0) * 8;
-            unsigned a1[4], a2[4];
-#pragma unroll
-            for (int k = 0; k < 4; ++k) { a1[k] = __vadd2(T[k], kc.K1[k]); if (GAP == CG) a2[k] = __vadd2(T[k], kc.K2[k]); }
-            const int off1 = e1 * jr0 - (GAP == LG ? 0 : oe1), off2 = e2 * jr0 - oe2;
-            int tot1, tot2 = 0;
-            int x1 = max(warp_excl_max(lane_max8(a1) + off1, lane, tot1), carry1);
-            carry1 = max(carry1, tot1);
-            const int xl1 = min(max(x1 - off1, NEGP), 32767);
-            unsigned P1[4], P2[4];
-            lane_excl_prefix(a1, pk(xl1, xl1), P1);
-            if (GAP == CG) {
-                int x2 = max(warp_excl_max(lane_max8(a2) + off2, lane, tot2), carry2);
-                carry2 = max(carry2, tot2);
-                const int xl2 = min(max(x2 - off2, NEGP), 32767);
-                lane_excl_prefix(a2, pk(xl2, xl2), P2);
-            }
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-                if (GAP == LG) {
-                    /* inclusive: H[c] = max(P[c], a[c]) - e1*c */
-                    unsigned h = __viaddmax_s16x2(__vmaxs2(P1[k], a1[k]), kc.KLG[k], NEGP2);
-                    if (MODE == LOCAL) h = __vmaxs2(h, zr2);
-                    H[k] = __vmins2(h, CAP[k]);
-                } else {
-                    F1[k] = __viaddmax_s16x2(P1[k], kc.KF1[k], NEGP2);
-                    if (GAP == AG) {
-                        const unsigned t = __vmaxs2(M[k], X1[k]);
-                        unsigned fz = F1[k];
-                        if (MODE == LOCAL) fz = __vmaxs2(fz, zr2);
-                        const unsigned h = __vmaxs2(t, fz);
-                        const unsigned from_t = __vcmpges2(t, fz);            /* h == t, per cell */
-                        const unsigned ev = __viaddmax_s16x2(X1[k], kc.NE1, __viaddmax_s16x2(h, kc.NOE1, NEGP2));
-                        const unsigned alt = (MODE == LOCAL) ? zr2 : NEGP2;
-                        E1o[k] = __vmins2((ev & from_t) | (alt & ~from_t), CAP[k]);
-                        H[k] = __vmins2(h, CAP[k]);
-                    } else {
-                        F2[k] = __viaddmax_s16x2(P2[k], kc.KF2[k], NEGP2);
-                        unsigned h = __vimax3_s16x2(T[k], F1[k], F2[k]);
-                        if (MODE == LOCAL) h = __vmaxs2(h, zr2);
-                        unsigned eo1 = __viaddmax_s16x2(X1[k], kc.NE1, __viaddmax_s16x2(h, kc.NOE1, NEGP2));
-                        unsigned eo2 = __viaddmax_s16x2(X2[k], kc.NE2, __viaddmax_s16x2(h, kc.NOE2, NEGP2));
-                        if (MODE == LOCAL) { eo1 = __vmaxs2(eo1, zr2); eo2 = __vmaxs2(eo2, zr2); }
-                        H[k] = __vmins2(h, CAP[k]); E1o[k] = __vmins2(eo1, CAP[k]); E2o[k] = __vmins2(eo2, CAP[k]);
-                    }
-                }
-            }
+            unsigned H[4], F1[4], F2[4], E1o[4], E2o[4];
+            p16_cells<GAP, MODE>(kc, CLO, CAP, S, M, X1, X2, (g - g0) * 8, e1, oe1, e2, oe2, zr2, lane, carry1, carry2, H, F1, F2, E1o, E2o);
 
             /* backtrace shortcut record (PoaBtRec): one bit per cell -- is H explained by the first predecessor's diagonal? */
             if (jd.btrec != nullptr) {
@@ -1489,39 +1624,6 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
                 if (lane == 0 && gp == g0)
                     *reinterpret_cast<uint4 *>(rec) = make_uint4((unsigned)(g0 * 8), (unsigned)mypred,
                                                                  (unsigned)rbase | (ngrp <= POA_BTREC_GROUPS ? 0x100u : 0u) | ((unsigned)min(ngrp, 0xffff) << 16), (unsigned)my_off);
-            }
-            /* FB: the insertion-step comparisons of the backtrace on the values stored for this row (exact: every value is
-             * >= NEGP and every penalty <= 1000 (poa_p16_ok), so the packed additions cannot wrap) */
-            uint2 fbits = make_uint2(0u, 0u);
-            if (RL::BITS) {
-                const unsigned hl = __shfl_up_sync(FULL, H[3], 1), f1l = __shfl_up_sync(FULL, F1[3], 1);
-                unsigned f2l = 0u;
-                if (GAP == CG) f2l = __shfl_up_sync(FULL, F2[3], 1);
-                const unsigned hp = lane == 0 ? fb_h : hl, f1p = lane == 0 ? fb_f1 : f1l, f2p = lane == 0 ? fb_f2 : f2l;
-                /* cell 8g-1 is inside the band exactly when g > g0 (beg lies in group g0) */
-                const unsigned clp = g > g0 ? 0x7fff0000u : 0u;
-                unsigned v[4];
-#pragma unroll
-                for (int k = 0; k < 4; ++k) {
-                    const unsigned inb = __vcmpeq2(CAP[k], 0x7fff7fffu);                          /* j in the band   */
-                    const unsigned inl = inb & __vcmpeq2(sh1(k ? CLO[k - 1] : clp, CLO[k]), 0x7fff7fffu);   /* and j-1 too */
-                    const unsigned hs = sh1(k ? H[k - 1] : hp, H[k]), fs1 = sh1(k ? F1[k - 1] : f1p, F1[k]);
-                    unsigned x = (__vcmpeq2(H[k], F1[k]) & inb & (FB_A * 0x10001u))
-                               | (__vcmpeq2(__vadd2(hs, kc.NOE1), F1[k]) & inl & (FB_B * 0x10001u))
-                               | (__vcmpeq2(__vadd2(fs1, kc.NE1), F1[k]) & inl & (FB_C * 0x10001u));
-                    if (GAP == CG) {
-                        const unsigned fs2 = sh1(k ? F2[k - 1] : f2p, F2[k]);
-                        x |= (__vcmpeq2(H[k], F2[k]) & inb & ((FB_A << 3) * 0x10001u))
-                           | (__vcmpeq2(__vadd2(hs, kc.NOE2), F2[k]) & inl & ((FB_B << 3) * 0x10001u))
-                           | (__vcmpeq2(__vadd2(fs2, kc.NE2), F2[k]) & inl & ((FB_C << 3) * 0x10001u));
-                    }
-                    v[k] = x;
-                }
-                fbits = make_uint2(__byte_perm(v[0], v[1], 0x6420), __byte_perm(v[2], v[3], 0x6420));
-                if (g1 - gp >= 32) {                            /* uniform: another pass follows */
-                    fb_h = __shfl_sync(FULL, H[3], 31); fb_f1 = __shfl_sync(FULL, F1[3], 31);
-                    if (GAP == CG) fb_f2 = __shfl_sync(FULL, F2[3], 31);
-                }
             }
             KP(2)
             if (TMA && tma_row) {
@@ -1556,7 +1658,6 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
                 if (GAP == CG) *reinterpret_cast<uint4 *>(q + (size_t)PL::E2 * gplane) = make_uint4(E2o[0], E2o[1], E2o[2], E2o[3]);
                 if (!FB && GAP != LG) *reinterpret_cast<uint4 *>(q + (size_t)PL::F1 * gplane) = make_uint4(F1[0], F1[1], F1[2], F1[3]);
                 if (!FB && GAP == CG) *reinterpret_cast<uint4 *>(q + (size_t)PL::F2 * gplane) = make_uint4(F2[0], F2[1], F2[2], F2[3]);
-                if (RL::BITS) *reinterpret_cast<uint2 *>(reinterpret_cast<uint8_t *>(rowp + (size_t)RL::N16 * gplane) + (size_t)rel * 8) = fbits;
             }
 
             KP(3)
@@ -1651,7 +1752,10 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
     if (lane == 0) *jd.result = res;
     __syncwarp();
     if (prm->ret_cigar && res.status == POA_ST_OK) {
-        poa_backtrack<GAP, ST, MODE, FB>(jv, jd, prm, mat_s, lane, best_i, best_j, *jd.result, 3, jd.btrec);
+        FbCtx fx;                                            /* FB: the ring is free now and holds the recomputed decision bytes */
+        fx.kc = &kc; fx.cap_lo = cap_lo; fx.cap_hi = cap_hi;
+        fx.buf = reinterpret_cast<uint8_t *>(ring_data); fx.buf_cells = (int)ring_row_bytes * ring_rows;
+        poa_backtrack<GAP, ST, MODE, FB>(jv, jd, prm, mat_s, lane, best_i, best_j, *jd.result, 3, jd.btrec, &fx);
         if (lane == 0) jd.result->bt_clk = clock64() - clk1;
     }
 }
