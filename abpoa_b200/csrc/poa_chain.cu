@@ -14,8 +14,9 @@
  * Groups the device cannot finish (capacity, int16 window, band wider than estimated) are reported
  * back and completed by the launch-per-round engine -- same results either way.
  *
- * Scope of the chain: global alignment, banded (wb >= 0), packed-int16 admissible scores, consensus
- * output (no per-edge read sets), unit base weights.  Everything else takes the other engine.
+ * Scope of the chain: global alignment, banded (wb >= 0), packed-int16 admissible scores, heaviest-bundling
+ * consensus and/or row-column MSA (one read set per node, not per edge), unit base weights.  Everything else
+ * takes the other engine.
  */
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -155,6 +156,36 @@ __global__ void __launch_bounds__(32) poa_chain_consensus_kernel(PoaChainSlot *s
     rec_off[blockIdx.x] = (int64_t)at;
 }
 
+/* RC-MSA of every finished group, one CTA per group: ranks on one thread (chain_msa_rank), rows by the whole CTA
+ * (chain_msa_rows).  with_cons: add the consensus row, from the path chain_consensus left in scr[1] -- run_cons: compute
+ * that path here (the consensus kernel did not run).  A record is [msa_len, n_rows, rows as bytes], packed through the
+ * same cursor as the consensus records, at word rec_base + cursor; rec_off[g] = -1 if the group has none (it is then
+ * finished by the launch engine). */
+__global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_msa_kernel(PoaChainSlot *slots, const PoaChainParams *cp, int n, int with_cons, int run_cons,
+                                                                    int32_t *out, unsigned long long *cursor, unsigned long long rec_base,
+                                                                    unsigned long long out_words, int64_t *rec_off) {
+    if ((int)blockIdx.x >= n) return;
+    __shared__ long long at_s;
+    __shared__ int len_s;
+    PoaChainSlot *s = &slots[blockIdx.x];
+    if (threadIdx.x == 0) {
+        if (run_cons && !s->failed && s->n_nodes >= 3) chain_consensus(s, cp, s->scr[2], s->n_cap);
+        const int msa_len = chain_msa_rank(s, cp);
+        long long at = -1;
+        if (msa_len > 0) {
+            const unsigned long long words = 2 + ((unsigned long long)(s->n_reads + with_cons) * (unsigned long long)msa_len + 3) / 4;
+            const unsigned long long a = rec_base + atomicAdd(cursor, words);
+            if (a + words <= out_words) at = (long long)a;
+        }
+        at_s = at; len_s = msa_len;
+        rec_off[blockIdx.x] = at;
+        if (at >= 0) { out[at] = msa_len; out[at + 1] = s->n_reads + with_cons; }
+    }
+    __syncthreads();
+    if (at_s < 0) return;
+    chain_msa_rows(s, cp, len_s, with_cons, reinterpret_cast<uint8_t *>(out + at_s + 2));
+}
+
 /* ------------------------------------------------------------------ host side */
 static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
@@ -164,7 +195,8 @@ int poa_chain_eligible(const abpoa_para_t *abpt) {
     { const char *np = getenv("ABPOA_GPU_NO_P16"); if (np && *np == '1') return 0; }      /* the chain only has the packed int16 kernel */
     if (abpt->align_mode != ABPOA_GLOBAL_MODE || abpt->wb < 0) return 0;
     if (abpt->gap_mode == ABPOA_LINEAR_GAP) return 0;                      /* banded linear gaps: generic kernel only (lane-exact band edges) */
-    if (abpt->use_read_ids || abpt->out_msa || abpt->out_gfa || abpt->max_n_cons > 1 || abpt->cons_algrm != ABPOA_HB) return 0;
+    /* RC-MSA runs on the chain (per-node read sets, poa_chain_msa_kernel); use_read_ids is what abpoa_post_set_para sets for it */
+    if ((abpt->use_read_ids && !abpt->out_msa) || abpt->out_gfa || abpt->max_n_cons > 1 || abpt->cons_algrm != ABPOA_HB) return 0;
     if (abpt->use_qv || abpt->amb_strand || abpt->inc_path_score || abpt->zdrop > 0 || abpt->rev_cigar || !abpt->ret_cigar) return 0;
     if (abpt->put_gap_on_right || abpt->put_gap_at_end) return 0;         /* handled by the kernels, but keep the chain on the common configuration */
     if (abpt->m > POA_MAX_M) return 0;
@@ -178,6 +210,7 @@ struct GroupPlan {
     int g;                  /* index into the caller's groups */
     int n_reads, qmax; int64_t bases;
     int n_cap; size_t static_bytes; double pool_units_est;
+    double rec_bytes;       /* RC-MSA runs: bound on the group's result records (0 otherwise) */
 };
 
 struct Cohort {
@@ -255,6 +288,11 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         return !serialised_launches;
     }();
     const double pool_margin = 1.15;
+    /* RC-MSA: one read set of W words per node (W of the largest group); the rows come back as records */
+    const bool want_msa = abpt->out_msa != 0;
+    const int with_cons = abpt->out_cons ? 1 : 0;
+    int W = 0;
+    if (want_msa) for (int g : todo) W = std::max(W, (groups[g].n_seq + 63) / 64);
 
     /* ---- per-group sizes ---- */
     std::vector<GroupPlan> plans;
@@ -291,7 +329,10 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         b += al256((size_t)m * ((((size_t)p.qmax + 1 + 7) & ~(size_t)7) + 8) * 2);  /* query profile   */
         b += al256(sizeof(PoaResultDev)) + al256(nc * sizeof(PoaBtRec));
         if (record) b += 2 * al256((size_t)p.n_reads * 4) + al256((size_t)p.n_reads * 8);
+        if (W > 0) b += al256(nc * W * 8);                         /* read sets      */
         p.static_bytes = b;
+        /* result records in the (then idle) plane pool: consensus + MSA rows, msa_len <= nodes */
+        p.rec_bytes = want_msa ? (double)(nc + 1) * 4 + 8 + (double)(p.n_reads + with_cons) * (double)nc + 1024 : 0.0;
         /* plane units of the group's largest (last) alignment.  Free-running, a group's slab is private and its rows take
          * what their bands really need: rows 3.2 % growth per read, 2w+1 cells plus the 8-cell grid per row (5 % error,
          * 50 x 10 kbp: 25.0k rows, 29-30.4 groups per row measured; estimate 25.8k x 30).  The round schedule bump-allocates
@@ -315,7 +356,7 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         size_t end = from, need_static = 0; double need_pool = 0;
         while (end < plans.size() && end - from < limit) {
             const size_t s2 = need_static + plans[end].static_bytes + sizeof(PoaChainSlot) + 4096;
-            const double p2 = need_pool + plans[end].pool_units_est * 16.0 * pool_margin;
+            const double p2 = need_pool + std::max(plans[end].pool_units_est * 16.0 * pool_margin, plans[end].rec_bytes);
             if (end > from && (double)s2 + p2 + (64 << 20) > (double)arena_cap) break;
             need_static = s2; need_pool = p2; ++end;
         }
@@ -394,6 +435,7 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
             s.jd.result = (PoaResultDev *)dtake(sizeof(PoaResultDev));
             s.jd.btrec = (PoaBtRec *)dtake(nc * sizeof(PoaBtRec));
             if (record) { s.rec_score = (int32_t *)dtake((size_t)p.n_reads * 4); s.rec_nops = (int32_t *)dtake((size_t)p.n_reads * 4); s.rec_hash = (uint64_t *)dtake((size_t)p.n_reads * 8); }
+            if (W > 0) s.read_set = (uint64_t *)dtake(nc * W * 8);
             if (p.n_reads > max_reads) max_reads = p.n_reads;
         }
         /* the read bytes themselves: half a gigabyte at BASELINE size, copied into the pinned buffer by all workers */
@@ -441,6 +483,7 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
             h_exoff[t] = ex_words; h_excap[t] = (int32_t)std::min<int64_t>(cap, INT32_MAX); ex_words += (cap + 63) & ~63ll;
         }
         int64_t *d_exoff = (int64_t *)dtake((size_t)nw * 8); int32_t *d_excap = (int32_t *)dtake((size_t)nw * 4);
+        int64_t *d_msaoff = want_msa ? (int64_t *)dtake((size_t)nw * 8) : NULL;          /* MSA record offsets */
         /* the export buffer and the plane pool share what is left: planes are dead when the export runs */
         doff = al256(doff);
         if (doff > total) poa_die("libabpoa_b200/chain", "wave layout (%zu bytes) exceeds the arena (%zu bytes)", doff, total);
@@ -473,7 +516,7 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         }
         PoaChainParams hcp; memset(&hcp, 0, sizeof hcp);
         hcp.K = K; hcp.A = A; hcp.m = m; hcp.max_mat = abpt->max_mat; hcp.min_mis = abpt->min_mis; hcp.o1 = abpt->gap_open1; hcp.e1 = abpt->gap_ext1;
-        hcp.oe1 = abpt->gap_open1 + abpt->gap_ext1; hcp.oe2 = abpt->gap_open2 + abpt->gap_ext2; hcp.record = record ? 1 : 0; hcp.P = P;
+        hcp.oe1 = abpt->gap_open1 + abpt->gap_ext1; hcp.oe2 = abpt->gap_open2 + abpt->gap_ext2; hcp.record = record ? 1 : 0; hcp.P = P; hcp.W = W;
         PoaParamsDev hprm; poa_fill_params(&hprm, abpt, 15);
 
         /* ---- upload (stream 0 of the wave), then fork the cohort streams ---- */
@@ -561,13 +604,21 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         const bool export_graph = [] { const char *e = getenv("ABPOA_GPU_CHAIN_EXPORT_GRAPH"); return e && *e == '1'; }();
         unsigned long long *d_ccur = d_cursors;               /* the pool cursors are idle now: reuse the first as the record cursor */
         int64_t *d_recoff = d_exoff;                          /* and the export offsets as record offsets */
+        /* RC-MSA: the rows are always the device's (poa_chain_msa_kernel); -r1 needs no consensus.  Its records share the
+         * consensus records' cursor, behind the export records when the graph comes back too. */
+        const bool cons_kernel = !export_graph && (!want_msa || with_cons);
+        const unsigned long long rec_base = export_graph ? (unsigned long long)ex_words : 0;
         if (export_graph) poa_chain_export_kernel<<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw, d_ex, d_exoff, d_excap);
-        else {
-            CK(cudaMemsetAsync(d_ccur, 0, sizeof(unsigned long long), s0));
-            poa_chain_consensus_kernel<<<nw, 32, 0, s0>>>(d_slots, d_cp, nw, d_ex, d_ccur, (unsigned long long)(pool_bytes / 4), d_recoff);
-        }
+        if (!export_graph || want_msa) CK(cudaMemsetAsync(d_ccur, 0, sizeof(unsigned long long), s0));
+        if (cons_kernel) poa_chain_consensus_kernel<<<nw, 32, 0, s0>>>(d_slots, d_cp, nw, d_ex, d_ccur, (unsigned long long)(pool_bytes / 4), d_recoff);
         CK(cudaGetLastError());
-        ++launches;
+        launches += (export_graph || cons_kernel) ? 1 : 0;
+        if (want_msa) {
+            poa_chain_msa_kernel<<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw, with_cons, export_graph && with_cons, d_ex, d_ccur, rec_base,
+                                                            (unsigned long long)(pool_bytes / 4), d_msaoff);
+            CK(cudaGetLastError());
+            ++launches;
+        }
         std::vector<PoaChainSlot> fin((size_t)nw);
         PoaChainSlot *h_fin = (PoaChainSlot *)pinned_get(1, (size_t)nw * sizeof(PoaChainSlot));
         CK(cudaMemcpyAsync(h_fin, d_slots, (size_t)nw * sizeof(PoaChainSlot), cudaMemcpyDeviceToHost, s0));
@@ -599,17 +650,20 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         }
         const double t_dev_done = now_ms();
         /* ---- device consensus: record offsets, then one copy of all records ---- */
-        std::vector<int64_t> recoff((size_t)nw, -1); int32_t *h_cons = NULL; unsigned long long cons_words = 0;
-        if (!export_graph) {
-            int64_t *h_ro = NULL; CK(cudaHostAlloc((void **)&h_ro, (size_t)nw * 8 + 8, cudaHostAllocDefault));
-            CK(cudaMemcpyAsync(h_ro, d_recoff, (size_t)nw * 8, cudaMemcpyDeviceToHost, s0));
-            CK(cudaMemcpyAsync(h_ro + nw, d_ccur, 8, cudaMemcpyDeviceToHost, s0));
+        std::vector<int64_t> recoff((size_t)nw, -1), msaoff((size_t)nw, -1); int32_t *h_cons = NULL; unsigned long long cons_words = 0;
+        if (!export_graph || want_msa) {           /* records: [rec_base, rec_base + cursor) words of d_ex */
+            int64_t *h_ro = NULL; CK(cudaHostAlloc((void **)&h_ro, (size_t)nw * 16 + 8, cudaHostAllocDefault));
+            if (cons_kernel) CK(cudaMemcpyAsync(h_ro, d_recoff, (size_t)nw * 8, cudaMemcpyDeviceToHost, s0));
+            if (want_msa) CK(cudaMemcpyAsync(h_ro + nw, d_msaoff, (size_t)nw * 8, cudaMemcpyDeviceToHost, s0));
+            CK(cudaMemcpyAsync(h_ro + 2 * nw, d_ccur, 8, cudaMemcpyDeviceToHost, s0));
             CK(cudaStreamSynchronize(s0));
-            memcpy(recoff.data(), h_ro, (size_t)nw * 8); cons_words = (unsigned long long)h_ro[nw];
+            if (cons_kernel) memcpy(recoff.data(), h_ro, (size_t)nw * 8);
+            if (want_msa) memcpy(msaoff.data(), h_ro + nw, (size_t)nw * 8);
+            cons_words = (unsigned long long)h_ro[2 * nw];
             CK(cudaFreeHost(h_ro));
-            if (cons_words > pool_bytes / 4) cons_words = pool_bytes / 4;
+            if (rec_base + cons_words > pool_bytes / 4) cons_words = pool_bytes / 4 - rec_base;
             h_cons = (int32_t *)pinned_get(2, (size_t)std::max<unsigned long long>(cons_words, 1) * 4);
-            if (cons_words) CK(cudaMemcpyAsync(h_cons, d_ex, (size_t)cons_words * 4, cudaMemcpyDeviceToHost, s0));
+            if (cons_words) CK(cudaMemcpyAsync(h_cons, d_ex + rec_base, (size_t)cons_words * 4, cudaMemcpyDeviceToHost, s0));
         }
         /* word counts: header words 0..3 of every record */
         std::vector<int32_t> hdr4((size_t)nw * 4);
@@ -622,8 +676,9 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
         }
         std::vector<int64_t> words((size_t)nw, 0), hoff2((size_t)nw, 0); int64_t tot_words = 0;
         for (int t = 0; t < nw; ++t) {
-            if (!export_graph) { words[t] = (!fin[t].failed && recoff[t] >= 0) ? 1 : 0; continue; }
-            if (fin[t].failed || hdr4[4 * t] < 2) continue;
+            const bool rec_ok = (!cons_kernel || recoff[t] >= 0) && (!want_msa || msaoff[t] >= 0);
+            if (!export_graph) { words[t] = (!fin[t].failed && rec_ok) ? 1 : 0; continue; }
+            if (fin[t].failed || hdr4[4 * t] < 2 || !rec_ok) continue;
             words[t] = 4 + 5ll * hdr4[4 * t] + 4ll * hdr4[4 * t + 1] + hdr4[4 * t + 2];
             hoff2[t] = tot_words; tot_words += words[t];
         }
@@ -669,12 +724,16 @@ int poa_chain_run(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_workers, 
                     abs->n_seq = p.n_reads; poa_seq_reserve(abs);
                     for (int i = 0; i < p.n_reads; ++i) { abs->is_rc[i] = 0; abs->name[i].l = 0; }
                     if (export_graph) poa_graph_import(ab, abpt, h_ex + hoff2[t]);
-                    else {                                     /* the device's consensus: base | coverage << 8 per position */
+                    else if (cons_kernel) {                    /* the device's consensus: base | coverage << 8 per position */
                         const int32_t *rec = h_cons + recoff[t];
                         const int len = rec[0];
                         std::vector<uint8_t> cb((size_t)(len > 0 ? len : 1)); std::vector<int> cc((size_t)(len > 0 ? len : 1));
                         for (int j = 0; j < len; ++j) { cb[j] = (uint8_t)(rec[1 + j] & 0xff); cc[j] = rec[1 + j] >> 8; }
                         poa_cons_install(ab, p.n_reads, len, cb.data(), cc.data());
+                    }
+                    if (want_msa) {                            /* the device's rows: [msa_len, n_rows, bytes] */
+                        const int32_t *rec = h_cons + (msaoff[t] - (int64_t)rec_base);
+                        poa_msa_install(ab, p.n_reads, rec[1], rec[0], reinterpret_cast<const uint8_t *>(rec + 2));
                     }
                     poa_finish_group_result(ab, abpt, o, emit, p.g);
                     o->dp_cells = fin[t].cells; o->n_aligned = p.n_reads - 1;

@@ -33,6 +33,7 @@
 #define POA_TID0 1
 #define POA_SHARED static
 #define POA_ATOMIC_OR(p, v) (*(p) |= (v))
+#define POA_CTZ64(x) __builtin_ctzll(x)
 #define POA_CHAIN_T 256
 #else
 #define POA_DEV __device__ __forceinline__
@@ -41,6 +42,7 @@
 #define POA_TID0 (threadIdx.x == 0)
 #define POA_SHARED __shared__
 #define POA_ATOMIC_OR(p, v) atomicOr((p), (v))
+#define POA_CTZ64(x) (__ffsll((long long)(x)) - 1)
 #define POA_CHAIN_T 256                 /* threads per CTA of the fuse kernel */
 #endif
 
@@ -62,6 +64,7 @@ typedef struct PoaChainParams {         /* one per batch call */
     int32_t record;                     /* keep per-read score / CIGAR length / FNV-1a hash */
     int32_t P;                          /* plane units per 8-cell group of a DP row (compact layout:
                                            H and the E planes; 1 / 2 / 3) */
+    int32_t W;                          /* 64-bit words per read set (ceil(n_reads / 64) of the largest group); 0: no RC-MSA */
 } PoaChainParams;
 
 typedef struct PoaChainSlot {           /* one per read group; every pointer aims into the group's HBM region */
@@ -99,6 +102,9 @@ typedef struct PoaChainSlot {           /* one per read group; every pointer aim
     int64_t btdiag[5];                  /* -DPOA_KPROF builds: PoaResultDev.btdiag summed */
     /* per-read records (record mode) */
     int32_t *rec_score, *rec_nops; uint64_t *rec_hash;
+    /* RC-MSA (PoaChainParams::W > 0): bit r of node v's set = read r's path passes through v, i.e. the union of the read
+     * sets of v's out-edges in the host graph -- all the row-column MSA needs (reference src/abpoa_output.c:105-192) */
+    uint64_t *read_set;                                 /* [n_cap * W] */
 } PoaChainSlot;
 
 /* Free-running chain: every group advances at its own pace.  One resident warp per group runs its alignments back to back;
@@ -360,6 +366,10 @@ POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
             order[i + 1] = v; s->node_row[v] = i + 1;
         }
     }
+    if (cp->W > 0) {                                     /* read 0 passes through SRC and every node it created; SINK has no out-edge */
+        const int W = cp->W;
+        POA_PAR_FOR(v, n) { uint64_t *rs = s->read_set + (size_t)v * W; for (int wd = 0; wd < W; ++wd) rs[wd] = (wd == 0 && v != 1) ? 1ull : 0ull; }
+    }
     if (POA_TID0) { s->n_nodes = n; s->cur = 0; s->fused = 1; s->retry = 0; }
     POA_CTA_SYNC();
     chain_set_remain(s, K, order, n);
@@ -502,6 +512,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
             const int id = old_n + newidx[qi];
             const int col = tgt[qi];                         /* CK_NEWM: the column's node */
             s->base[id] = seq[qi]; s->in_cnt[id] = 0; s->out_cnt[id] = 0; s->aln_cnt[id] = 0; s->n_read[id] = 0;
+            if (cp->W > 0) for (int wd = 0; wd < cp->W; ++wd) s->read_set[(size_t)id * cp->W + wd] = 0;
             new_anchor[newidx[qi]] = kind_anchor[qi] & 0x0fffffff;      /* compacted: by new-node rank (anchors are non-decreasing) */
             item_row[qi] = col;                              /* remember the column for the aligned-set update */
             tgt[qi] = id;
@@ -536,6 +547,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
             }
         }
         s->n_read[from] += 1;
+        if (cp->W > 0) s->read_set[(size_t)from * cp->W + (r >> 6)] |= 1ull << (r & 63);      /* item qi owns node `from` */
     }
     POA_CTA_SYNC();
 
@@ -629,6 +641,86 @@ POA_DEV void chain_consensus(PoaChainSlot *s, const PoaChainParams *cp, int32_t 
         out[1 + len++] = (int32_t)s->base[cur] | (s->n_read[cur] << 8);
     }
     out[0] = len;
+}
+
+/* ------------------------------------------------------------------ row-column MSA on the device
+ * Ranks (host twin: poa_set_msa_rank in poa_graph.c): Kahn from SRC with a LIFO stack; a node is pushed, together with
+ * its aligned set, when its in-degree and that of every aligned sibling have reached 0; a popped node without a rank
+ * takes the next one together with its aligned set.  Out-edges and aligned sets are visited in list order, which is the
+ * host's order node for node.  Serial, on one thread per group (like chain_consensus).  Leaves rank[] in scr[5] and
+ * returns msa_len = rank[SINK] - 1, or -1. */
+POA_DEV int chain_msa_rank(PoaChainSlot *s, const PoaChainParams *cp) {
+    if (!POA_TID0) return -1;
+    const int K = cp->K, A = cp->A, n = s->n_nodes;
+    int32_t *deg = s->scr[3], *st = s->scr[4], *rank = s->scr[5];
+    if (s->failed || n < 3) return -1;
+    for (int v = 0; v < n; ++v) deg[v] = s->in_cnt[v];
+    int top = 0, next_rank = 0;
+    st[top++] = 0; rank[0] = -1;
+    while (top > 0) {
+        const int cur = st[--top];
+        const int na = s->aln_cnt[cur];
+        const int32_t *al = s->aln_id + (size_t)cur * A;
+        if (rank[cur] < 0) {
+            rank[cur] = next_rank;
+            for (int a = 0; a < na; ++a) rank[al[a]] = next_rank;
+            ++next_rank;
+        }
+        if (cur == 1) return rank[1] - 1;
+        const int ne = s->out_cnt[cur];
+        const int32_t *oid = s->out_id + (size_t)cur * K;
+        for (int e = 0; e < ne; ++e) {
+            const int v = oid[e];
+            if (--deg[v] != 0) continue;
+            const int nv = s->aln_cnt[v];
+            const int32_t *av = s->aln_id + (size_t)v * A;
+            int ready = 1;
+            for (int a = 0; a < nv; ++a) if (deg[av[a]] != 0) { ready = 0; break; }
+            if (!ready) continue;
+            if (top + 1 + nv > n) return -1;                  /* every node is pushed once: a graph that breaks this is not a DAG */
+            st[top++] = v; rank[v] = -1;
+            for (int a = 0; a < nv; ++a) { st[top++] = av[a]; rank[av[a]] = -1; }
+        }
+    }
+    return -1;
+}
+
+/* Rows of the RC-MSA (host twin: abpoa_generate_rc_msa in poa_cons.c) from the ranks of chain_msa_rank: n_reads rows (+ the
+ * consensus row if with_cons) of msa_len codes, gaps = cp->m.  The column of a node is the largest rank in its aligned set,
+ * minus one.  Every node id >= 2 writes its base into the rows of the reads in its read set; the consensus row takes the
+ * consensus path chain_consensus left in scr[1] (nxt).  Needs the whole CTA. */
+POA_DEV void chain_msa_rows(PoaChainSlot *s, const PoaChainParams *cp, int msa_len, int with_cons, uint8_t *rows) {
+    const int A = cp->A, W = cp->W, n = s->n_nodes, nr = s->n_reads;
+    const int32_t *rank = s->scr[5], *nxt = s->scr[1];
+    int32_t *col = s->scr[4];                            /* the rank pass's stack is dead */
+    POA_PAR_FOR(v, n) {
+        int r = rank[v];
+        const int32_t *al = s->aln_id + (size_t)v * A;
+        for (int a = 0; a < s->aln_cnt[v]; ++a) if (rank[al[a]] > r) r = rank[al[a]];
+        col[v] = r - 1;
+    }
+    for (int i = 0; i < nr + with_cons; ++i) {
+        uint8_t *row = rows + (size_t)i * msa_len;
+        POA_PAR_FOR(j, msa_len) row[j] = (uint8_t)cp->m;   /* code m prints as '-' */
+    }
+    POA_CTA_SYNC();
+    POA_PAR_FOR(v, n) {
+        if (v >= 2) {                                    /* every node is ranked before SINK, which takes the last rank */
+            const uint8_t b = s->base[v];
+            const size_t c = (size_t)col[v];
+            const uint64_t *rs = s->read_set + (size_t)v * W;
+            for (int wd = 0; wd < W; ++wd)
+                for (uint64_t bits = rs[wd]; bits; bits &= bits - 1) {
+                    const int rd = wd * 64 + POA_CTZ64(bits);
+                    rows[(size_t)rd * msa_len + c] = b;
+                }
+        }
+    }
+    if (with_cons && POA_TID0) {
+        uint8_t *row = rows + (size_t)nr * msa_len;
+        for (int cur = nxt[0]; cur != 1 && cur >= 0; cur = nxt[cur]) row[col[cur]] = s->base[cur];
+    }
+    POA_CTA_SYNC();
 }
 
 #endif

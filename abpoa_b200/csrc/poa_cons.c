@@ -131,6 +131,20 @@ void poa_cons_install(abpoa_t *ab, int n_seq, int len, const uint8_t *base, cons
     ab->abg->is_called_cons = 1;
 }
 
+/* RC-MSA rows that were computed elsewhere (the device chain, poa_chain.cuh: chain_msa_rows) installed as the handle's
+ * result.  Install a device consensus first (poa_cons_install clears abc).  With no graph on the host,
+ * abpoa_generate_rc_msa returns at once; with an imported graph it keeps these rows. */
+void poa_msa_install(abpoa_t *ab, int n_seq, int n_rows, int msa_len, const uint8_t *rows) {
+    abpoa_cons_t *abc = ab->abc;
+    abc->n_seq = n_seq; abc->msa_len = msa_len;
+    abc->msa_base = (uint8_t **)poa_xmalloc((size_t)n_rows * sizeof(uint8_t *));
+    for (int i = 0; i < n_rows; ++i) {
+        abc->msa_base[i] = (uint8_t *)poa_xmalloc((size_t)POA_MAX(msa_len, 1));
+        memcpy(abc->msa_base[i], rows + (size_t)i * msa_len, (size_t)msa_len);
+    }
+    poa_graph_set_msa_installed(ab->abg);
+}
+
 /* column of a node = max rank over its aligned group, 1-based */
 static int msa_column(const abpoa_graph_t *abg, int id) {
     int r = abg->node_id_to_msa_rank[id];
@@ -142,7 +156,7 @@ static int msa_column(const abpoa_graph_t *abg, int id) {
 void abpoa_generate_rc_msa(abpoa_t *ab, abpoa_para_t *abpt) {
     abpoa_graph_t *abg = ab->abg;
     poa_graph_sync_public(abg);
-    if (abg->node_n <= 2) return;
+    if (abg->node_n <= 2 || poa_graph_msa_installed(abg)) return;
     poa_set_msa_rank(abg, ABPOA_SRC_NODE_ID, ABPOA_SINK_NODE_ID);
     if (abpt->out_cons) abpoa_generate_consensus(ab, abpt);
 

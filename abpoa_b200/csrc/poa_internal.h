@@ -53,6 +53,10 @@ void poa_cons_clear(abpoa_cons_t *abc);            /* free members, keep the str
 void poa_cons_free(abpoa_cons_t *abc);
 void poa_set_msa_rank(abpoa_graph_t *abg, int src_id, int sink_id);
 void poa_cons_install(abpoa_t *ab, int n_seq, int len, const uint8_t *base, const int *cov);   /* a consensus computed on the device */
+/* RC-MSA rows computed on the device: n_rows rows of msa_len codes back to back (n_seq reads, then the consensus row) */
+void poa_msa_install(abpoa_t *ab, int n_seq, int n_rows, int msa_len, const uint8_t *rows);
+int poa_graph_msa_installed(const abpoa_graph_t *abg);  /* abc holds installed rows for the current graph */
+void poa_graph_set_msa_installed(abpoa_graph_t *abg);
 int poa_edge_path_score(const abpoa_graph_t *abg, int node_id, int in_idx);  /* -G scores */
 /* dense, node-id-indexed views kept by poa_graph.c (see poa_graph_x) */
 void poa_graph_sync_public(abpoa_graph_t *abg);        /* fold dense n_read / n_span_read into node[] */
