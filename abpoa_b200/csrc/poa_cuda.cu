@@ -691,6 +691,105 @@ extern "C" int poa_debug_last_run(abpoa_t *ab, int32_t *out8) {
     return 0;
 }
 
+/* debugging aid: replay the most recent single alignment of `ab` on the chain engine's job function (the compact row layout,
+ * p16_run_job<GAP, GLOBAL, LEAN, no TMA, FB> on one warp, as poa_chain_dp_worker_kernel runs it) and rebuild every row's F
+ * planes with the backtrace's recompute (poa_launch_fb_dump).  The job's blob, parameters and query profile are the ones
+ * the alignment left on the device; the replay gets its own row records, a slab of the full rectangle, CIGAR, backtrace
+ * records and result, so the five-plane run stays readable with poa_debug_fetch_planes.
+ *   ring_rows, ring_cells  ring geometry of the replay; 0, 0: what the chain picks for this job's band (28 KB budget)
+ *   buf_cells              decision-byte buffer of the recompute: > 0 as given, 0: the chain's (its ring), < 0: a whole row
+ * Outputs, one copy each: rowinfo[4 * n_rows] (beg, end, left, right), rowoff[n_rows] (8-cell units), the compact slab,
+ * the F slab (int16, a row's F1 (, F2) at its slab offset, ngrp * 8 cells each), the decision bytes (one per cell at the
+ * row's slab offset: cap / 2 bytes), the graph-CIGAR (node ids, in abpoa_res_t order) and out[16] = status, best score,
+ * node_e, query_e, node_s, query_s, n_ops, cells, max_band, plane_units_used, ring_rows, ring_cells, buf_cells,
+ * windows recomputed (all rows), windows of the row with the most.
+ * Returns -1 unless the last accepted run was the packed LEAN global kernel with affine or convex gaps, -2 for a ring that
+ * does not fit one CTA or a buffer that does not fit shared memory; else the slab capacity the outputs need (bytes) when
+ * `slab` is NULL or `cap` is smaller, else the bytes of the compact slab the replay used.  Nothing of the chain's or the
+ * launch engine's own path runs here. */
+extern "C" cudaError_t poa_launch_chain_replay(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int ring_rows, int ring_cells,
+                                               cudaStream_t st);
+extern "C" cudaError_t poa_launch_fb_dump(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int n_rows, int buf_cells,
+                                          int16_t *fslab, uint8_t *fbits, int32_t *windows, cudaStream_t st);
+extern "C" int poa_chain_fb_buf_cells(int gap_mode, int ring_rows, int ring_cells);
+extern "C" int64_t poa_debug_chain_replay(abpoa_t *ab, int ring_rows, int ring_cells, int buf_cells, int32_t *rowinfo, uint32_t *rowoff,
+                                          void *slab, void *fslab, uint8_t *fbits, int64_t cap, uint64_t *cigar, int64_t cigar_cap, int64_t *out16) {
+    poa_dev_ctx *c = (poa_dev_ctx *)ab->abm->s_mem;
+    if (!c || c->arena || c->last_rows <= 0 || c->last_bits != 15 || !c->last_lean) return -1;
+    if (c->last_gap != ABPOA_AFFINE_GAP && c->last_gap != ABPOA_CONVEX_GAP) return -1;
+    CK(cudaSetDevice(c->dev));
+    PoaJobHeader hd; CK(cudaMemcpy(&hd, c->last_desc.blob, sizeof hd, cudaMemcpyDeviceToHost));
+    const int n_rows = hd.n_rows, qlen = hd.qlen, gap = c->last_gap;
+    const int n16 = gap == ABPOA_AFFINE_GAP ? 2 : 3;
+    const uint64_t units = (uint64_t)((qlen + 1 + 7) / 8 + 1) * n16 * n_rows;      /* full rectangle: no PLANE_OVF */
+    const int64_t need = (int64_t)units * POA_GROUP * 2;
+    if (!slab || cap < need) return need;
+    if (ring_rows <= 0 || ring_cells <= 0) {
+        const int band_cells = hd.w >= 0 ? (2 * hd.w + 1 + 104 + 7) / 8 * 8 : (qlen + 1 + 7) / 8 * 8 + 8;
+        poa_pick_ring(gap, 16, band_cells, (size_t)28 * 1024, &ring_rows, &ring_cells);
+    }
+    PoaParamsDev prm; CK(cudaMemcpy(&prm, c->d_in, sizeof prm, cudaMemcpyDeviceToHost));     /* what the alignment ran with */
+    const int gaps[4] = { prm.e1, prm.oe1, prm.e2, prm.oe2 };
+    /* fresh outputs: result | rowinfo | rowoff | cigar | btrec | slab | F slab | bytes | windows */
+    const size_t o_ri = al256(sizeof(PoaResultDev)), o_ro = o_ri + al256((size_t)n_rows * sizeof(PoaRowInfo));
+    const size_t o_cg = o_ro + al256((size_t)n_rows * sizeof(PoaRowOff)), cg_cap = (size_t)qlen + n_rows + 8;
+    const size_t o_bt = o_cg + al256(cg_cap * 8), o_sl = o_bt + al256((size_t)n_rows * sizeof(PoaBtRec));
+    const size_t o_fs = o_sl + al256((size_t)need), o_fb = o_fs + al256((size_t)need), o_wn = o_fb + al256((size_t)need / 2);
+    const size_t total = o_wn + al256((size_t)n_rows * 4);
+    uint8_t *d = NULL;
+    CK(cudaMalloc((void **)&d, total));
+    CK(cudaMemset(d, 0, total));
+    PoaJobDesc jd = c->last_desc;
+    jd.result = (PoaResultDev *)d; jd.rowinfo = (PoaRowInfo *)(d + o_ri); jd.rowoff = (PoaRowOff *)(d + o_ro);
+    jd.cigar = (uint64_t *)(d + o_cg); jd.cigar_cap = (int32_t)cg_cap; jd.btrec = (PoaBtRec *)(d + o_bt);
+    jd.planes = d + o_sl; jd.plane_cap_units = units;
+    const cudaError_t le = poa_launch_chain_replay(gap, gaps, &jd, (const PoaParamsDev *)c->d_in, ring_rows, ring_cells, c->st);
+    if (le == cudaErrorInvalidValue) { cudaGetLastError(); CK(cudaFree(d)); return -2; }
+    CK(le);
+    PoaResultDev r; CK(cudaMemcpyAsync(&r, d, sizeof r, cudaMemcpyDeviceToHost, c->st));
+    std::vector<PoaRowInfo> ri(n_rows); std::vector<PoaRowOff> ro(n_rows);
+    CK(cudaMemcpyAsync(ri.data(), d + o_ri, (size_t)n_rows * sizeof(PoaRowInfo), cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(ro.data(), d + o_ro, (size_t)n_rows * sizeof(PoaRowOff), cudaMemcpyDeviceToHost, c->st));
+    stream_wait(c);
+    int max_ngrp = 1;
+    for (int i = 0; i < n_rows - 1; ++i) if (ri[i].end >= ri[i].beg) max_ngrp = std::max(max_ngrp, (ri[i].end >> 3) - (ri[i].beg >> 3) + 1);
+    if (buf_cells == 0) buf_cells = poa_chain_fb_buf_cells(gap, ring_rows, ring_cells);
+    else if (buf_cells < 0) buf_cells = (max_ngrp + 31) / 32 * 256;
+    std::vector<int32_t> win(n_rows, 0);
+    if (r.status == POA_ST_OK) {                        /* every row record is written: the dump reads inside the slab only */
+        const cudaError_t de = poa_launch_fb_dump(gap, gaps, &jd, (const PoaParamsDev *)c->d_in, n_rows, buf_cells, (int16_t *)(d + o_fs), d + o_fb,
+                                                  (int32_t *)(d + o_wn), c->st);
+        if (de == cudaErrorInvalidValue) { cudaGetLastError(); CK(cudaFree(d)); return -2; }
+        CK(de);
+        CK(cudaMemcpyAsync(fslab, d + o_fs, (size_t)need, cudaMemcpyDeviceToHost, c->st));
+        CK(cudaMemcpyAsync(fbits, d + o_fb, (size_t)need / 2, cudaMemcpyDeviceToHost, c->st));
+        CK(cudaMemcpyAsync(win.data(), d + o_wn, (size_t)n_rows * 4, cudaMemcpyDeviceToHost, c->st));
+    }
+    const int n_ops = r.status == POA_ST_OK ? r.n_ops : 0;
+    std::vector<uint64_t> ops((size_t)std::max(n_ops, 1));
+    if (n_ops > 0) CK(cudaMemcpyAsync(ops.data(), d + o_cg, (size_t)n_ops * 8, cudaMemcpyDeviceToHost, c->st));
+    CK(cudaMemcpyAsync(slab, d + o_sl, (size_t)need, cudaMemcpyDeviceToHost, c->st));
+    stream_wait(c);
+    CK(cudaFree(d));
+    for (int i = 0; i < n_rows; ++i) {
+        rowinfo[4 * i] = ri[i].beg; rowinfo[4 * i + 1] = ri[i].end; rowinfo[4 * i + 2] = ri[i].left; rowinfo[4 * i + 3] = ri[i].right;
+        rowoff[i] = ro[i].off;
+    }
+    /* the device names graph positions by DP row (whole-graph job: row = node index); as poa_job_to_res */
+    const int *id_of_row = ab->abg->index_to_node_id;
+    for (int t = 0; t < n_ops && t < cigar_cap; ++t) {
+        uint64_t w = ops[n_ops - 1 - t];
+        if ((w & 0xf) != ABPOA_CINS) w = ((uint64_t)id_of_row[w >> 34] << 34) | (w & 0x3ffffffffull);
+        cigar[t] = w;
+    }
+    int64_t wsum = 0, wmax = 0;
+    for (int i = 0; i < n_rows; ++i) { wsum += win[i]; wmax = std::max<int64_t>(wmax, win[i]); }
+    const int64_t o[16] = { r.status, r.best_score, id_of_row[r.best_i], r.best_j - 1, id_of_row[r.start_i], r.start_j - 1, n_ops, r.cells, r.max_band,
+                            (int64_t)r.plane_units_used, ring_rows, ring_cells, buf_cells, wsum, wmax, 0 };
+    memcpy(out16, o, sizeof o);
+    return (int64_t)r.plane_units_used * POA_GROUP * 2;
+}
+
 /* debugging aid: redo launches (PLANE_OVF / RANGE) of the handle's single-alignment context so far */
 extern "C" int64_t poa_debug_retries(abpoa_t *ab) {
     poa_dev_ctx *c = (poa_dev_ctx *)ab->abm->s_mem;

@@ -194,7 +194,10 @@ struct FbCtx {
     const P16Consts *kc; const uint4 *cap_lo, *cap_hi;   /* the packed kernel's constants and band-mask tables          */
     uint8_t *buf; int buf_cells;                          /* decision bytes of one row: the shared-memory ring, idle now */
 };
-template <int GAP, int MODE>
+/* fb_recompute<..., DUMP = true> (debug export poa_debug_chain_replay only): also stores the recomputed F1 (/ F2) of the
+ * kept passes, F1 of group g at f + 8 (g - g0), F2 fstride cells later -- the row's F planes as the five-plane layout holds them */
+struct FbDumpCtx : FbCtx { int16_t *f; int fstride; };
+template <int GAP, int MODE, bool DUMP = false>
 __device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaParamsDev *prm, const FbCtx &fx,
                             int beg, int end, int pb, int np, int base, int j, int lane);
 
@@ -1158,7 +1161,7 @@ __device__ __forceinline__ uint2 p16_fbits(const P16Consts &kc, const unsigned H
  * (p16_cells), fed from the predecessors' H / E planes in HBM, the query profile and the band-mask tables, pass by pass from
  * the band's first cell to cell j.  The decision bytes of the last fx.buf_cells / 256 passes up to j's go to fx.buf, from the
  * returned cell on.  Jobs of the compact layout run the LEAN forward pass, which has no path scores (chain jobs carry none). */
-template <int GAP, int MODE>
+template <int GAP, int MODE, bool DUMP>
 __device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaParamsDev *prm, const FbCtx &fx,
                             int beg, int end, int pb, int np, int base, int j, int lane) {
     const P16Consts &kc = *fx.kc;
@@ -1225,6 +1228,14 @@ __device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaPa
         p16_cells<GAP, MODE>(kc, CLO, CAP, S, M, X1, X2, (g - g0) * 8, e1, oe1, e2, oe2, zr2, lane, carry1, carry2, H, F1, F2, E1o, E2o);
         const uint2 bits = p16_fbits<GAP>(kc, H, F1, F2, CLO, CAP, g > g0, lane, p < pj, lh, lf1, lf2);
         if (p >= p_lo && active) *reinterpret_cast<uint2 *>(fx.buf + (g * 8 - lo)) = bits;
+        if constexpr (DUMP) {
+            if (p >= p_lo && active) {
+                const FbDumpCtx &dx = static_cast<const FbDumpCtx &>(fx);
+                int16_t *q = dx.f + (size_t)(g - g0) * POA_GROUP;
+                *reinterpret_cast<uint4 *>(q) = make_uint4(F1[0], F1[1], F1[2], F1[3]);
+                if (GAP == CG) *reinterpret_cast<uint4 *>(q + dx.fstride) = make_uint4(F2[0], F2[1], F2[2], F2[3]);
+            }
+        }
     }
     __syncwarp();
     return lo;
@@ -1913,6 +1924,94 @@ extern "C" cudaError_t poa_launch_chain_align_p16(int gap_mode, const int *gaps,
     if (gap_mode == LG) return launch_chain_one<LG>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
     if (gap_mode == AG) return launch_chain_one<AG>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
     return launch_chain_one<CG>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
+}
+
+/* ------------------------------------------------------------------ debug: the chain's job function on one job
+ * (poa_debug_chain_replay in poa_cuda.cu, for the tests).  The replay kernel makes the call poa_chain_dp_worker_kernel
+ * makes, on a job the host hands over with fresh output buffers.  The dump kernel (one warp per row 1 .. n_rows - 2)
+ * then rebuilds every row's F planes with the backtrace's fb_recompute, right to left the way the insertion steps walk: at
+ * the row's last cell first, then at the cell left of the previous window, down to the band's first cell.  It keeps the
+ * decision bytes as the backtrace reads them back from the buffer, bits[off * 8 + (j - 8 g0)] for a row stored at
+ * plane offset off, and the F values at the same offsets in an int16 slab (F1, then F2, ngrp * 8 cells each). */
+template <int GAP>
+__global__ void POA_P16_BOUNDS poa_chain_replay_kernel(const __grid_constant__ PoaJobDesc jd, const PoaParamsDev *__restrict__ prm,
+                                                       int ring_rows, int ring_cells, const __grid_constant__ P16Consts kc) {
+    extern __shared__ __align__(16) uint8_t dyn_smem[];
+    const int lane = threadIdx.x;
+    const P16Smem sm = p16_smem_init(dyn_smem, prm, ring_rows, lane);
+    p16_run_job<GAP, GLOBAL, true, false, true>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
+}
+
+template <int GAP>
+__global__ void __launch_bounds__(32) poa_fb_dump_kernel(const __grid_constant__ PoaJobDesc jd, const PoaParamsDev *__restrict__ prm, int buf_cells,
+                                                         int16_t *fslab, uint8_t *fbits, int32_t *windows, const __grid_constant__ P16Consts kc) {
+    extern __shared__ __align__(16) uint8_t dyn_smem[];
+    const int lane = threadIdx.x, i = blockIdx.x + 1;
+    const JobView jv = open_job(jd.blob);
+    if (i >= jv.n_rows - 1) return;
+    const P16Smem sm = p16_smem_init(dyn_smem, prm, 0, lane);            /* no ring: the byte buffer follows the mask tables */
+    const PoaRowInfo ri = jd.rowinfo[i];
+    int n = 0;
+    if (ri.end >= ri.beg) {
+        const uint32_t off = jd.rowoff[i].off;
+        const int g0 = ri.beg >> 3, ngrp = (ri.end >> 3) - g0 + 1;
+        FbDumpCtx fx;
+        fx.kc = &kc; fx.cap_lo = sm.cap_lo; fx.cap_hi = sm.cap_hi;
+        fx.buf = reinterpret_cast<uint8_t *>(sm.ring_data); fx.buf_cells = buf_cells;
+        fx.f = fslab + (size_t)off * POA_GROUP; fx.fstride = ngrp * POA_GROUP;
+        const int2 m0 = ldb(jv.rowmeta + i);
+        const int np = ldb(&jv.rowmeta[i + 1].x) - m0.x;
+        uint8_t *ob = fbits + (size_t)off * POA_GROUP;
+        for (int j = ri.end; j >= ri.beg; ++n) {
+            const int lo = fb_recompute<GAP, GLOBAL, true>(jv, jd, prm, fx, ri.beg, ri.end, m0.x, np, m0.y & 0xff, j, lane);
+            for (int c = lo + lane; c <= j; c += 32) ob[c - g0 * 8] = fx.buf[c - lo];
+            __syncwarp();
+            j = lo - 1;
+        }
+    }
+    if (lane == 0) windows[i] = n;
+}
+
+/* largest dynamic shared memory of one CTA (sm_90) */
+#define POA_SMEM_MAX (227 * 1024)
+template <int GAP>
+static cudaError_t launch_chain_replay_one(const PoaJobDesc &jd, const PoaParamsDev *prm, int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
+    const size_t smem = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
+    if (smem > POA_SMEM_MAX) return cudaErrorInvalidValue;
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_replay_kernel<GAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, POA_SMEM_MAX);
+    if (e != cudaSuccess) return e;
+    poa_chain_replay_kernel<GAP><<<1, 32, smem, st>>>(jd, prm, ring_rows, ring_cells, kc);
+    return cudaGetLastError();
+}
+/* ring_rows: a power of two >= 2; ring_cells: a positive multiple of 8 (poa_pick_ring gives no less); their ring must fit one CTA */
+extern "C" cudaError_t poa_launch_chain_replay(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int ring_rows, int ring_cells,
+                                               cudaStream_t st) {
+    if (gap_mode == LG || ring_rows < 2 || (ring_rows & (ring_rows - 1)) || ring_cells < 8 || (ring_cells & 7)) return cudaErrorInvalidValue;
+    const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
+    if (gap_mode == AG) return launch_chain_replay_one<AG>(*jd, prm, ring_rows, ring_cells, kc, st);
+    return launch_chain_replay_one<CG>(*jd, prm, ring_rows, ring_cells, kc, st);
+}
+/* the bytes of the chain's backtrace buffer for a ring geometry (fx.buf_cells in p16_run_job) */
+extern "C" int poa_chain_fb_buf_cells(int gap_mode, int ring_rows, int ring_cells) {
+    const int rn = gap_mode == LG ? RingPlanes<LG>::N : (gap_mode == AG ? RingPlanes<AG>::N : RingPlanes<CG>::N);
+    return rn * ring_cells * 2 * ring_rows;
+}
+template <int GAP>
+static cudaError_t launch_fb_dump_one(const PoaJobDesc &jd, const PoaParamsDev *prm, int n_rows, int buf_cells, int16_t *fslab, uint8_t *fbits,
+                                      int32_t *windows, const P16Consts &kc, cudaStream_t st) {
+    const size_t smem = (size_t)POA_MAX_M * POA_MAX_M * sizeof(int) + 18 * sizeof(uint4) + (size_t)std::max(buf_cells >> 8, 1) * 256;
+    if (smem > POA_SMEM_MAX) return cudaErrorInvalidValue;
+    cudaError_t e = cudaFuncSetAttribute(poa_fb_dump_kernel<GAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, POA_SMEM_MAX);
+    if (e != cudaSuccess) return e;
+    if (n_rows > 2) poa_fb_dump_kernel<GAP><<<n_rows - 2, 32, smem, st>>>(jd, prm, buf_cells, fslab, fbits, windows, kc);
+    return cudaGetLastError();
+}
+extern "C" cudaError_t poa_launch_fb_dump(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int n_rows, int buf_cells,
+                                          int16_t *fslab, uint8_t *fbits, int32_t *windows, cudaStream_t st) {
+    if (gap_mode == LG) return cudaErrorInvalidValue;
+    const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
+    if (gap_mode == AG) return launch_fb_dump_one<AG>(*jd, prm, n_rows, buf_cells, fslab, fbits, windows, kc, st);
+    return launch_fb_dump_one<CG>(*jd, prm, n_rows, buf_cells, fslab, fbits, windows, kc, st);
 }
 
 /* ------------------------------------------------------------------ launcher */

@@ -49,6 +49,9 @@ def _bind(lib):
         d.poa_debug_fetch_planes.argtypes = [capi.abpoa_t_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64]
         d.poa_debug_last_run.restype = C.c_int
         d.poa_debug_last_run.argtypes = [capi.abpoa_t_p, C.c_void_p]
+        d.poa_debug_chain_replay.restype = C.c_int64
+        d.poa_debug_chain_replay.argtypes = [capi.abpoa_t_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                             C.c_int64, C.c_void_p, C.c_int64, C.c_void_p]
         d._planes_bound = True
     return d
 
@@ -95,6 +98,68 @@ def fetch_planes(session: PoaSession, info: RunInfo):
     return rowinfo, rowoff, slab[:need].view(np.int32 if info.kernel == 32 else np.int16)
 
 
+@dataclass
+class ChainReplay:
+    """The last alignment replayed on the chain engine's job function (poa_debug_chain_replay): compact row layout
+    (H, E1 (, E2)), then every row's F planes and insertion-step decision bytes rebuilt by the backtrace's recompute."""
+    status: int
+    best_score: int
+    ends: tuple                    # (node_s, node_e, query_s, query_e), as abpoa_res_t holds them
+    n_ops: int
+    cells: int
+    max_band: int
+    plane_units_used: int
+    ring_rows: int
+    ring_cells: int
+    buf_cells: int                 # decision-byte buffer of the recompute (cells)
+    windows: int                   # fb_recompute calls of the dump, all rows
+    max_windows: int               # ... of the row with the most
+    cigar: np.ndarray              # graph-CIGAR (node ids)
+    rowinfo: np.ndarray            # [n_rows, 4] beg, end, left, right
+    rowoff: np.ndarray             # [n_rows] slab offset of each row (8-cell units)
+    slab: np.ndarray               # int16: H, E1 (, E2) of each row, ngrp * 8 cells each
+    fslab: np.ndarray              # int16: F1 (, F2) of each row at the same offsets
+    fbits: np.ndarray              # uint8: decision byte of cell j of a row at rowoff * 8 + j - 8 (beg >> 3)
+
+
+def chain_replay(session: PoaSession, info: RunInfo, qlen: int, ring_rows: int = 0, ring_cells: int = 0, buf_cells: int = 0) -> ChainReplay:
+    """Replay the last alignment of `session` with ring geometry (ring_rows, ring_cells) (0, 0: the chain's pick) and a
+    recompute buffer of buf_cells cells (0: the chain's, the ring; -1: a whole row)."""
+    d = _bind(session.lib)
+    out = np.zeros(16, dtype=np.int64)
+    need = d.poa_debug_chain_replay(session.ab, ring_rows, ring_cells, buf_cells, None, None, None, None, None, 0, None, 0, out.ctypes.data)
+    assert need > 0, f"poa_debug_chain_replay refused the last alignment ({need})"
+    rowinfo = np.zeros((info.n_rows, 4), dtype=np.int32)
+    rowoff = np.zeros(info.n_rows, dtype=np.uint32)
+    slab = np.zeros(need // 2, dtype=np.int16)
+    fslab = np.zeros(need // 2, dtype=np.int16)
+    fbits = np.zeros(need // 2, dtype=np.uint8)
+    cig = np.zeros(qlen + info.n_rows + 8, dtype=np.uint64)
+    used = d.poa_debug_chain_replay(session.ab, ring_rows, ring_cells, buf_cells, rowinfo.ctypes.data, rowoff.ctypes.data, slab.ctypes.data,
+                                    fslab.ctypes.data, fbits.ctypes.data, need, cig.ctypes.data, len(cig), out.ctypes.data)
+    assert used >= 0, f"poa_debug_chain_replay: geometry ({ring_rows}, {ring_cells}) / buffer {buf_cells} rejected ({used})"
+    o = [int(x) for x in out]
+    return ChainReplay(o[0], o[1], (o[4], o[2], o[5], o[3]), o[6], o[7], o[8], o[9], o[10], o[11], o[12], o[13], o[14], cig[:o[6]].copy(),
+                       rowinfo, rowoff, slab, fslab, fbits)
+
+
+def decision_bytes(h: np.ndarray, fs: list, gaps: list) -> np.ndarray:
+    """The insertion-step decision byte of every cell of one row's band (RowLayout in poa_kernels.cu) from the row's H and F
+    planes over the band: for F plane k with penalties (oe_k, e_k), bits 3k .. 3k+2 are
+      FB_A  H[j] == F_k[j],   FB_B  H[j-1] - oe_k == F_k[j],   FB_C  F_k[j-1] - e_k == F_k[j]
+    with B and C 0 at the band's first cell.  In int64, so no value wraps."""
+    h = np.asarray(h, dtype=np.int64)
+    out = np.zeros(len(h), dtype=np.uint8)
+    for k, (f, (oe, e)) in enumerate(zip(fs, gaps)):
+        f = np.asarray(f, dtype=np.int64)
+        a = h == f
+        b = np.zeros(len(h), dtype=bool); c = np.zeros(len(h), dtype=bool)
+        b[1:] = h[:-1] - oe == f[1:]
+        c[1:] = f[:-1] - e == f[1:]
+        out |= ((a * 1 | b * 2 | c * 4) << (3 * k)).astype(np.uint8)
+    return out
+
+
 def oracle_rows_of(align):
     """Run `align(row_cb)` and collect the oracle's rows: {row: (beg, end, [H, E1, E2, F1, F2] or None each)}."""
     rows = {}
@@ -113,17 +178,25 @@ def score_bits(abpt, qlen: int, n_rows: int) -> int:
     return 16 if max_score <= 32767 - a.min_mis - (a.gap_open1 + a.gap_ext1) - (a.gap_open2 + a.gap_ext2) else 32
 
 
-def compare_planes(session: PoaSession, rows: dict, info: RunInfo, qlen: int, tag: str = "") -> list[str]:
+# product plane k holds oracle plane PLANE_ORDER[n_planes][k] (five-plane layout of each gap mode)
+PLANE_ORDER = {1: (0,), 3: (0, 1, 3), 5: (0, 1, 2, 3, 4)}
+
+
+def compare_planes(session: PoaSession, rows: dict, info: RunInfo, qlen: int, tag: str = "", order=None, planes=None) -> list[str]:
     """Every rule of the module docstring on the last alignment of `session`; returns the violations (at most one per
-    row and plane, each naming row, plane and column), [] when the planes match."""
+    row and plane, each naming row, plane and column), [] when the planes match.
+    order: the oracle plane (index into PLANE_NAMES) of each plane a row stores, in storage order; default PLANE_ORDER of
+    the kernel's plane count.  planes: (rowinfo, rowoff, slab) to check instead of fetch_planes(session, info), e.g. the
+    compact slab (H, E1 (, E2)) or the recomputed F slab (F1 (, F2)) of the chain's job function (ChainReplay)."""
     cfg = session.cfg
     # storage granule of a row (log2 cells): the 8-cell group, except banded linear-gap rows outside local mode on the
     # generic kernel ("lgx"), which are stored in whole reference vectors of pn = 16 / 8 cells around the band
     lgx = info.kernel != 15 and session.abpt.contents.gap_mode == ABPOA_LINEAR_GAP and cfg.align_mode != ABPOA_LOCAL_MODE and cfg.wb >= 0
     xs = (4 if score_bits(session.abpt, qlen, info.n_rows) == 16 else 3) if lgx else 3
-    rowinfo, rowoff, slab = fetch_planes(session, info)
+    rowinfo, rowoff, slab = fetch_planes(session, info) if planes is None else planes
     floor = FLOOR[info.kernel]
-    order = {1: [0], 3: [0, 1, 3], 5: [0, 1, 2, 3, 4]}[info.n_planes]    # product plane k holds oracle plane order[k]
+    order = PLANE_ORDER[info.n_planes] if order is None else tuple(order)
+    n_planes = len(order)
     with_argmax = cfg.wb >= 0 or cfg.align_mode != ABPOA_GLOBAL_MODE
     bad = []
     for row in sorted(rows):
@@ -150,7 +223,7 @@ def compare_planes(session: PoaSession, rows: dict, info: RunInfo, qlen: int, ta
         ngrp = (((((end >> xs) + 1) << xs) - 1) >> 3) - g0 + 1
         info.widest_groups = max(info.widest_groups, ngrp)
         base = int(rowoff[row]) * 8
-        stored = slab[base: base + info.n_planes * ngrp * 8].astype(np.int64).reshape(info.n_planes, ngrp * 8)
+        stored = slab[base: base + n_planes * ngrp * 8].astype(np.int64).reshape(n_planes, ngrp * 8)
         lo = beg - g0 * 8
         for k, pi in enumerate(order):
             want = pl[pi]
@@ -195,10 +268,12 @@ def _add_sub(session, r, res, beg_id, end_id, i, n):
         capi.libc_free(res.graph_cigar)
 
 
-def run_planes(cfg, reads, lib=None, windows=None, tag: str = "", check=None) -> PlanesRun:
+def run_planes(cfg, reads, lib=None, windows=None, tag: str = "", check=None, after=None) -> PlanesRun:
     """Progressive alignment of `reads` on the GPU with every DP plane compared to the oracle's after every read.
     windows: per read (inc_beg, inc_end) node-id windows for sub-graph alignment (abpoa_subgraph_nodes), or None.
     check(i, RunInfo): called after every aligned read (assert the kernel variant here).
+    after(session, oracle rows, RunInfo, oracle ReadAlignment): called after check, before the read joins the graph (more
+    checks on the same alignment, e.g. a replay of it with chain_replay).
     Raises AssertionError naming the first read / row / plane / column that differs."""
     from oracle_binding import oracle_align
     lib = lib or capi.product()
@@ -231,6 +306,8 @@ def run_planes(cfg, reads, lib=None, windows=None, tag: str = "", check=None) ->
                 out.runs.append(info)
                 if check is not None:
                     check(i, info)
+                if after is not None:
+                    after(gpu, rows, info, o)
             if windows is None:
                 gpu.add(r, res, len(reads)); cpu.add(r, ores, len(reads))
             else:
