@@ -107,6 +107,40 @@ typedef struct PoaChainSlot {           /* one per read group; every pointer aim
     uint64_t *read_set;                                 /* [n_cap * W] */
 } PoaChainSlot;
 
+/* A group's memory, host side: the slot's capacities and every per-group array, taken in one fixed order from the
+ * caller's allocator `take(bytes)`, which also decides the alignment.  The engine carves a wave's HBM with it, its
+ * wave planner sums the same requests, and the CPU emulator lays out its host buffer with it, so the three cannot
+ * disagree.  The reads (chain_slot_reads) live in a region of their own: they are staged and uploaded in one copy. */
+template <class Take>
+static inline void chain_slot_layout(PoaChainSlot *s, int n_cap, int qmax, int n_reads, int K, int A, int m, int W, bool record, Take take) {
+    const size_t nc = (size_t)n_cap, scr_n = nc > (size_t)qmax + 2 ? nc : (size_t)qmax + 2;
+    s->n_cap = n_cap; s->pred_cap = (int32_t)(nc * 3); s->n_reads = n_reads;
+    s->blob_cap = (int32_t)(256 + (nc + 1) * 8 + (size_t)s->pred_cap * 4 + 4 + (size_t)qmax + 64);
+    s->jd.cigar_cap = (int32_t)(qmax + n_cap + 8);
+    s->base = (uint8_t *)take(nc);
+    s->in_cnt = (int32_t *)take(nc * 4); s->out_cnt = (int32_t *)take(nc * 4); s->aln_cnt = (int32_t *)take(nc * 4); s->n_read = (int32_t *)take(nc * 4);
+    s->in_id = (int32_t *)take(nc * K * 4); s->in_w = (int32_t *)take(nc * K * 4); s->out_id = (int32_t *)take(nc * K * 4); s->out_w = (int32_t *)take(nc * K * 4);
+    s->aln_id = (int32_t *)take(nc * A * 4);
+    s->order[0] = (int32_t *)take(nc * 4); s->order[1] = (int32_t *)take(nc * 4); s->node_row = (int32_t *)take(nc * 4); s->rem_row = (int32_t *)take(nc * 4);
+    for (int k = 0; k < 6; ++k) s->scr[k] = (int32_t *)take(scr_n * 4);
+    s->jd.blob = (uint8_t *)take((size_t)s->blob_cap);
+    s->jd.rowinfo = (PoaRowInfo *)take(nc * sizeof(PoaRowInfo)); s->jd.rowoff = (PoaRowOff *)take(nc * sizeof(PoaRowOff));
+    s->jd.cigar = (uint64_t *)take((size_t)s->jd.cigar_cap * 8);
+    s->jd.qprof = (int16_t *)take((size_t)m * ((((size_t)qmax + 1 + 7) & ~(size_t)7) + 8) * 2);
+    s->jd.result = (PoaResultDev *)take(sizeof(PoaResultDev));
+    s->jd.btrec = (PoaBtRec *)take(nc * sizeof(PoaBtRec));
+    if (record) { s->rec_score = (int32_t *)take((size_t)n_reads * 4); s->rec_nops = (int32_t *)take((size_t)n_reads * 4); s->rec_hash = (uint64_t *)take((size_t)n_reads * 8); }
+    if (W > 0) s->read_set = (uint64_t *)take(nc * W * 8);
+}
+
+/* the group's reads: `bases` bytes back to back, n_reads + 1 offsets, n_reads band half widths */
+template <class Take>
+static inline void chain_slot_reads(PoaChainSlot *s, int n_reads, int64_t bases, Take take) {
+    s->reads = (const uint8_t *)take((size_t)bases);
+    s->read_off = (const int32_t *)take(((size_t)n_reads + 1) * 4);
+    s->read_w = (const int32_t *)take((size_t)n_reads * 4);
+}
+
 /* Free-running chain: every group advances at its own pace.  One resident warp per group runs its alignments back to back;
  * after each one it appends the group to `tasks` and waits; persistent fuse CTAs draw tickets, fuse + flatten the group and
  * hand it back.  `total` = fuse tasks that will ever be appended (lowered when a group leaves the chain early): a worker

@@ -11,48 +11,42 @@
 
 struct Emul {
     PoaChainSlot s; PoaChainParams cp;
-    std::vector<uint8_t> mem, blob, reads; std::vector<int32_t> read_off, read_w;
-    std::vector<uint64_t> cigar; PoaResultDev res;
-    std::vector<int32_t> rec_score, rec_nops; std::vector<uint64_t> rec_hash;
+    std::vector<uint8_t> mem;                              /* the group's arrays and reads, laid out by chain_slot_layout / chain_slot_reads */
 };
 
+/* W > 0: RC-MSA on, W words per read set */
 extern "C" Emul *chain_emul_new(int n_reads, const int32_t *lens, const uint8_t *const *seqs, const int32_t *w, int n_cap, int K, int A,
-                                int m, int max_mat, int min_mis, int o1, int e1, int oe1, int oe2) {
+                                int m, int max_mat, int min_mis, int o1, int e1, int oe1, int oe2, int W) {
     Emul *e = new Emul();
-    memset(&e->s, 0, sizeof e->s); memset(&e->cp, 0, sizeof e->cp); memset(&e->res, 0, sizeof e->res);
+    memset(&e->s, 0, sizeof e->s); memset(&e->cp, 0, sizeof e->cp);
     e->cp.K = K; e->cp.A = A; e->cp.m = m; e->cp.max_mat = max_mat; e->cp.min_mis = min_mis; e->cp.o1 = o1; e->cp.e1 = e1; e->cp.oe1 = oe1; e->cp.oe2 = oe2; e->cp.record = 1;
-    int qmax = 1; e->read_off.push_back(0);
-    for (int i = 0; i < n_reads; ++i) { e->reads.insert(e->reads.end(), seqs[i], seqs[i] + lens[i]); e->read_off.push_back((int32_t)e->reads.size()); e->read_w.push_back(w[i]); if (lens[i] > qmax) qmax = lens[i]; }
+    e->cp.W = W;
+    int qmax = 1; int64_t bases = 0;
+    for (int i = 0; i < n_reads; ++i) { bases += lens[i]; if (lens[i] > qmax) qmax = lens[i]; }
     PoaChainSlot &s = e->s;
-    s.n_cap = n_cap; s.pred_cap = n_cap * 4; s.n_reads = n_reads;
-    const size_t scr_n = (size_t)(qmax + 2 > n_cap ? qmax + 2 : n_cap);
-    size_t bytes = (size_t)n_cap * (1 + 4 * 4 + 4 * K * 4 + A * 4 + 4 * 4) + 6 * scr_n * 4 + 4096;
+    size_t bytes = 0;
+    auto count = [&](size_t b) { bytes += (b + 15) & ~(size_t)15; return (uint8_t *)NULL; };
+    chain_slot_layout(&s, n_cap, qmax, n_reads, K, A, m, W, true, count);
+    chain_slot_reads(&s, n_reads, bases, count);
     e->mem.assign(bytes, 0xcd);                            /* poison: nothing may rely on zeroed memory */
     uint8_t *p = e->mem.data();
     auto take = [&](size_t b) { uint8_t *q = p; p += (b + 15) & ~(size_t)15; return q; };
-    s.base = take(n_cap);
-    s.in_cnt = (int32_t *)take((size_t)n_cap * 4); s.out_cnt = (int32_t *)take((size_t)n_cap * 4); s.aln_cnt = (int32_t *)take((size_t)n_cap * 4); s.n_read = (int32_t *)take((size_t)n_cap * 4);
-    s.in_id = (int32_t *)take((size_t)n_cap * K * 4); s.in_w = (int32_t *)take((size_t)n_cap * K * 4);
-    s.out_id = (int32_t *)take((size_t)n_cap * K * 4); s.out_w = (int32_t *)take((size_t)n_cap * K * 4);
-    s.aln_id = (int32_t *)take((size_t)n_cap * A * 4);
-    s.order[0] = (int32_t *)take((size_t)n_cap * 4); s.order[1] = (int32_t *)take((size_t)n_cap * 4);
-    s.node_row = (int32_t *)take((size_t)n_cap * 4); s.rem_row = (int32_t *)take((size_t)n_cap * 4);
-    for (int k = 0; k < 6; ++k) s.scr[k] = (int32_t *)take(scr_n * 4);
-    s.blob_cap = (int32_t)(256 + ((size_t)n_cap + 1) * 8 + (size_t)s.pred_cap * 4 + qmax + 64);
-    e->blob.assign((size_t)s.blob_cap, 0xcd);
-    e->cigar.assign((size_t)qmax + n_cap + 8, 0);
-    s.reads = e->reads.data(); s.read_off = e->read_off.data(); s.read_w = e->read_w.data();
-    s.jd.blob = e->blob.data(); s.jd.cigar = e->cigar.data(); s.jd.result = &e->res;
-    e->rec_score.assign(n_reads, 0); e->rec_nops.assign(n_reads, 0); e->rec_hash.assign(n_reads, 0);
-    s.rec_score = e->rec_score.data(); s.rec_nops = e->rec_nops.data(); s.rec_hash = e->rec_hash.data();
+    chain_slot_layout(&s, n_cap, qmax, n_reads, K, A, m, W, true, take);
+    chain_slot_reads(&s, n_reads, bases, take);
+    uint8_t *reads = const_cast<uint8_t *>(s.reads);
+    int32_t *off = const_cast<int32_t *>(s.read_off), *rw = const_cast<int32_t *>(s.read_w);
+    off[0] = 0;
+    for (int i = 0; i < n_reads; ++i) { memcpy(reads + off[i], seqs[i], (size_t)lens[i]); off[i + 1] = off[i] + lens[i]; rw[i] = w[i]; }
     return e;
 }
 extern "C" void chain_emul_free(Emul *e) { delete e; }
 extern "C" void chain_emul_seed(Emul *e) { chain_seed(&e->s, &e->cp); }
 /* ops: graph-CIGAR words in BACKTRACK order with DP rows (what the alignment kernel leaves in jd.cigar) */
 extern "C" int chain_emul_fuse(Emul *e, const uint64_t *ops, int n_ops, int best_score, int64_t cells) {
-    memcpy(e->cigar.data(), ops, (size_t)n_ops * 8);
-    e->res.status = POA_ST_OK; e->res.n_ops = n_ops; e->res.best_score = best_score; e->res.cells = cells;
+    memcpy(e->s.jd.cigar, ops, (size_t)n_ops * 8);
+    PoaResultDev *res = e->s.jd.result;                    /* what the alignment kernel reports */
+    memset(res, 0, sizeof *res);
+    res->status = POA_ST_OK; res->n_ops = n_ops; res->best_score = best_score; res->cells = cells;
     chain_fuse(&e->s, &e->cp, e->s.fused);
     return e->s.failed;
 }
@@ -70,7 +64,7 @@ extern "C" const int32_t *chain_emul_array(Emul *e, int which) {
     return NULL;
 }
 extern "C" const uint8_t *chain_emul_bases(Emul *e) { return e->s.base; }
-extern "C" const uint8_t *chain_emul_blob(Emul *e) { return e->blob.data(); }
-extern "C" const uint64_t *chain_emul_hashes(Emul *e) { return e->rec_hash.data(); }
+extern "C" const uint8_t *chain_emul_blob(Emul *e) { return e->s.jd.blob; }
+extern "C" const uint64_t *chain_emul_hashes(Emul *e) { return e->s.rec_hash; }
 extern "C" int64_t chain_emul_cells(Emul *e) { return e->s.cells; }
 extern "C" int chain_emul_consensus(Emul *e, int32_t *out, int cap) { chain_consensus(&e->s, &e->cp, out, cap); return out[0]; }

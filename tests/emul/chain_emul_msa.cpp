@@ -3,14 +3,6 @@
  * suite can compare it with the host graph layer.  Nothing in the product links this file. */
 #include "chain_emul.cpp"
 
-/* RC-MSA on: W words per read set (poisoned, nothing may rely on zeroed memory); call before chain_emul_seed */
-extern "C" void chain_emul_enable_msa(Emul *e, int W) {
-    e->cp.W = W;
-    const size_t n = (size_t)e->s.n_cap * W;
-    e->s.read_set = (uint64_t *)malloc(n * sizeof(uint64_t) + 8);
-    for (size_t i = 0; i < n; ++i) e->s.read_set[i] = 0xcdcdcdcdcdcdcdcdull;
-}
-extern "C" void chain_emul_msa_free(Emul *e) { free(e->s.read_set); chain_emul_free(e); }
 extern "C" const uint64_t *chain_emul_read_set(Emul *e) { return e->s.read_set; }
 extern "C" const int32_t *chain_emul_msa_ranks(Emul *e) { return e->s.scr[5]; }
 /* ranks + rows after the last read, as poa_chain_msa_kernel runs them (with_cons: chain_consensus first, for its path);

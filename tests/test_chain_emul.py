@@ -31,7 +31,7 @@ def emul():
         subprocess.run(["g++", "-O1", "-g", "-fPIC", "-shared", f"-I{ROOT / 'abpoa_b200' / 'csrc'}", f"-I{ROOT / 'include'}", "-o", str(SO), str(src)], check=True)
     d = C.CDLL(str(SO))
     d.chain_emul_new.restype = C.c_void_p
-    d.chain_emul_new.argtypes = [C.c_int, c_int_p, C.POINTER(c_u8_p), c_int_p] + [C.c_int] * 10
+    d.chain_emul_new.argtypes = [C.c_int, c_int_p, C.POINTER(c_u8_p), c_int_p] + [C.c_int] * 11
     d.chain_emul_free.argtypes = [C.c_void_p]
     d.chain_emul_seed.argtypes = [C.c_void_p]
     d.chain_emul_fuse.restype = C.c_int
@@ -69,7 +69,7 @@ def drive(emul, product_lib, cfg: PoaConfig, reads, K=12, A=None, n_cap=None):
         a = s.abpt.contents
         ws = (C.c_int * n)(*[(-1 if a.wb < 0 else a.wb + int(np.float32(a.wf) * np.float32(len(x)))) for x in arrs])
         e = d.chain_emul_new(n, lens, ptrs, ws, n_cap, K, A, a.m, a.max_mat, a.min_mis, a.gap_open1, a.gap_ext1,
-                             a.gap_open1 + a.gap_ext1, a.gap_open2 + a.gap_ext2)
+                             a.gap_open1 + a.gap_ext1, a.gap_open2 + a.gap_ext2, 0)
         try:
             s.reset(max(len(x) for x in arrs))
             s.lib.dll.poa_graph_set_fast_order(s.ab.contents.abg, 1)

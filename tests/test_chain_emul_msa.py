@@ -34,13 +34,12 @@ def emul():
                         "-o", str(SO), str(srcs[0])], check=True)
     d = C.CDLL(str(SO))
     d.chain_emul_new.restype = C.c_void_p
-    d.chain_emul_new.argtypes = [C.c_int, c_int_p, C.POINTER(c_u8_p), c_int_p] + [C.c_int] * 10
-    d.chain_emul_msa_free.argtypes = [C.c_void_p]
+    d.chain_emul_new.argtypes = [C.c_int, c_int_p, C.POINTER(c_u8_p), c_int_p] + [C.c_int] * 11
+    d.chain_emul_free.argtypes = [C.c_void_p]
     d.chain_emul_seed.argtypes = [C.c_void_p]
     d.chain_emul_fuse.restype = C.c_int
     d.chain_emul_fuse.argtypes = [C.c_void_p, C.POINTER(C.c_uint64), C.c_int, C.c_int, C.c_int64]
     d.chain_emul_n_nodes.argtypes = [C.c_void_p]
-    d.chain_emul_enable_msa.argtypes = [C.c_void_p, C.c_int]
     d.chain_emul_read_set.restype = C.POINTER(C.c_uint64)
     d.chain_emul_read_set.argtypes = [C.c_void_p]
     d.chain_emul_msa_ranks.restype = c_int_p
@@ -77,9 +76,8 @@ def drive_msa(d, product_lib, cfg: PoaConfig, reads, K=12, extra_words=0):
         a = s.abpt.contents
         ws = (C.c_int * n)(*[(-1 if a.wb < 0 else a.wb + int(np.float32(a.wf) * np.float32(len(x)))) for x in arrs])
         e = d.chain_emul_new(n, lens, ptrs, ws, n_cap, K, A, a.m, a.max_mat, a.min_mis, a.gap_open1, a.gap_ext1,
-                             a.gap_open1 + a.gap_ext1, a.gap_open2 + a.gap_ext2)
+                             a.gap_open1 + a.gap_ext1, a.gap_open2 + a.gap_ext2, W)
         try:
-            d.chain_emul_enable_msa(e, W)
             s.reset(max(len(x) for x in arrs))
             s.lib.dll.poa_graph_set_fast_order(s.ab.contents.abg, 1)
             for i, r in enumerate(arrs):
@@ -124,7 +122,7 @@ def drive_msa(d, product_lib, cfg: PoaConfig, reads, K=12, extra_words=0):
                     assert np.array_equal(row, w), f"with_cons={with_cons}: MSA row {k} differs at column {int(np.argmax(row != w))}"
                 assert (buf[len(want_rows) * msa_len:] == 0xee).all(), "rows written past the record"
         finally:
-            d.chain_emul_msa_free(e)
+            d.chain_emul_free(e)
 
 
 @pytest.mark.parametrize("name", CHAIN_CASES)
