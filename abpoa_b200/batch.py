@@ -73,6 +73,9 @@ def _bind(lib):
     d.abpoa_gpu_msa_batch.argtypes = [C.c_void_p, capi.abpoa_para_t_p, C.c_int, C.POINTER(abpoa_gpu_group_t),
                                       C.POINTER(abpoa_gpu_group_result_t), C.c_int]
     d.abpoa_gpu_group_result_free.argtypes = [C.POINTER(abpoa_gpu_group_result_t)]
+    d.abpoa_gpu_msa_batch_write.restype = C.c_int
+    d.abpoa_gpu_msa_batch_write.argtypes = [C.c_void_p, capi.abpoa_para_t_p, C.c_int, C.POINTER(abpoa_gpu_group_t), C.c_void_p, C.c_void_p,
+                                            C.POINTER(abpoa_gpu_group_result_t), C.c_int]
     d.abpoa_gpu_batch_get_stats.argtypes = [C.c_void_p, C.POINTER(abpoa_gpu_stats_t)]
     d.abpoa_gpu_batch_reset_stats.argtypes = [C.c_void_p]
     d.abpoa_gpu_replay.restype = C.c_int
@@ -139,6 +142,17 @@ class BatchEngine:
         res = (abpoa_gpu_group_result_t * packed.n)()
         flags = (ABPOA_GPU_RECORD_READS if record_reads else 0) | (ABPOA_GPU_CAPTURE_JOBS if capture else 0) | (ABPOA_GPU_NO_CHAIN if no_chain else 0)
         self.d.abpoa_gpu_msa_batch(self.h, abpt, packed.n, packed.arr, res, flags)
+        return self._results(packed, res, record_reads, keep_results)
+
+    def run_write(self, abpt, packed: PackedGroups, out_fp, record_reads: bool = False, no_chain: bool = False):
+        """abpoa_gpu_msa_batch_write: the batch's output text (what abpoa_output prints per group, reads unnamed) goes to
+        the C stream `out_fp` (a FILE *, e.g. from libc fopen); returns the result records as run_packed does."""
+        res = (abpoa_gpu_group_result_t * packed.n)()
+        flags = (ABPOA_GPU_RECORD_READS if record_reads else 0) | (ABPOA_GPU_NO_CHAIN if no_chain else 0)
+        self.d.abpoa_gpu_msa_batch_write(self.h, abpt, packed.n, packed.arr, None, out_fp, res, flags)
+        return self._results(packed, res, record_reads, True)
+
+    def _results(self, packed, res, record_reads, keep_results):
         out = []
         for g in range(packed.n):
             r = res[g]

@@ -3,7 +3,7 @@
  * FASTA/FASTQ file per line = one read group per line) is exactly the batched shape the GPU wants, so all
  * files are read first and go through ONE abpoa_gpu_msa_batch_write call; the output is what the reference
  * prints file by file.  Options whose subsystems are outside the hot-path scope (-S/-p seeding, -i restore,
- * -r3/-r4 GFA, -g plot, -d>1, -a1, -L) are accepted and then refused by the library with a message. */
+ * -g plot, -d>1, -a1, -L) are accepted and then refused by the library with a message. */
 #include <getopt.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -38,7 +38,8 @@ static int usage(void) {
         "  -Q --use-qual-weight   -c --amino-acid\n"
         "  -l --in-list          the input is a list of files, one read group per file (all groups run as one GPU batch)\n"
         "  -o --output FILE      [stdout]\n"
-        "  -r --result INT       0: consensus FASTA, 1: RC-MSA, 2: both, 5: consensus FASTQ [0]\n"
+        "  -r --result INT       0: consensus FASTA, 1: RC-MSA, 2: both, 3: GFA, 4: GFA with consensus path,\n"
+        "                        5: consensus FASTQ [0]\n"
         "  -h --help  -v --version  -V --verbose INT\n\n", CLI_VERSION);
     return 1;
 }

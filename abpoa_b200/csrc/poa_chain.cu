@@ -15,8 +15,8 @@
  *                              and under tools that serialise kernel launches (profilers, sanitizers), where two kernels
  *                              that wait for each other cannot both run.
  *
- * The results come from the device: poa_chain_consensus_kernel (heaviest bundling) and poa_chain_msa_kernel (row-column
- * MSA) write records that come back in one copy and are installed into the caller's records.  With
+ * The results come from the device: poa_chain_consensus_kernel (heaviest bundling), poa_chain_msa_kernel (row-column
+ * MSA) and poa_chain_gfa_kernel (GFA) write records that come back in one copy and are installed into the caller's records.  With
  * ABPOA_GPU_CHAIN_EXPORT_GRAPH=1 the whole graph comes back instead (poa_chain_export_kernel, rebuilt by
  * poa_graph_import) and the host computes the consensus on it: the cross-check of the device graph against the host
  * code.  Groups the device cannot finish (capacity, int16 window, plane slab) are reported back and completed by the
@@ -27,7 +27,7 @@
  * (poa_chain.cuh) for the planner and the carve alike.
  *
  * Scope of the chain: global alignment, banded (wb >= 0), packed-int16 admissible scores, heaviest-bundling
- * consensus and/or row-column MSA (one read set per node, not per edge), unit base weights.  Everything else
+ * consensus, row-column MSA and GFA (one read set per node, not per edge), unit base weights.  Everything else
  * takes the other engine.
  */
 #include <cuda_runtime.h>
@@ -60,6 +60,7 @@ extern "C" void poa_pick_ring(int gap_mode, int bits, int band_cells, size_t sme
 
 static_assert(offsetof(PoaChainSync, q_tail) == 128 && offsetof(PoaChainSync, total) == 256 && offsetof(PoaChainSync, abort) == 384,
               "every polled / bumped word of PoaChainSync sits in its own 128-byte line");
+static_assert(POA_GFA_HDR_WORDS == POA_GFA_HDR, "the device's GFA record header is the one poa_gfa_from_record reads");
 
 /* ------------------------------------------------------------------ kernels */
 __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_seed_kernel(PoaChainSlot *slots, const PoaChainParams *cp, int n) {
@@ -199,6 +200,34 @@ __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_msa_kernel(PoaChainSlot
     chain_msa_rows(s, cp, len_s, with_cons, reinterpret_cast<uint8_t *>(out + at_s + 2));
 }
 
+/* GFA of every finished group, one CTA per group: order and size on one thread (chain_gfa_size), the record by the
+ * whole CTA (chain_gfa_record).  with_cons: the record carries the consensus path chain_consensus left in scr[1] --
+ * run_cons: compute that path here (the consensus kernel did not run).  Records share the consensus records' cursor at
+ * word rec_base + cursor, each 8-byte aligned; rec_off[g] = -1 if the group has none (it is then finished by the launch
+ * engine). */
+__global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_gfa_kernel(PoaChainSlot *slots, const PoaChainParams *cp, int n, int with_cons, int run_cons,
+                                                                    int32_t *out, unsigned long long *cursor, unsigned long long rec_base,
+                                                                    unsigned long long out_words, int64_t *rec_off) {
+    if ((int)blockIdx.x >= n) return;
+    __shared__ long long at_s;
+    __shared__ int32_t hdr_s[POA_GFA_HDR_WORDS];
+    PoaChainSlot *s = &slots[blockIdx.x];
+    if (threadIdx.x == 0) {
+        if (run_cons && !s->failed && s->n_nodes >= 3) chain_consensus(s, cp, s->scr[2], s->n_cap);
+        const long long words = chain_gfa_size(s, cp, with_cons, hdr_s);
+        long long at = -1;
+        if (words > 0) {
+            const unsigned long long a = (rec_base + atomicAdd(cursor, (unsigned long long)words + 1) + 1) & ~1ull;
+            if (a + (unsigned long long)words <= out_words) at = (long long)a;
+        }
+        at_s = at;
+        rec_off[blockIdx.x] = at;
+    }
+    __syncthreads();
+    if (at_s < 0) return;
+    chain_gfa_record(s, cp, hdr_s, out + at_s);
+}
+
 /* ------------------------------------------------------------------ host side */
 static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
 
@@ -208,8 +237,9 @@ int poa_chain_eligible(const abpoa_para_t *abpt) {
     { const char *np = getenv("ABPOA_GPU_NO_P16"); if (np && *np == '1') return 0; }      /* the chain only has the packed int16 kernel */
     if (abpt->align_mode != ABPOA_GLOBAL_MODE || abpt->wb < 0) return 0;
     if (abpt->gap_mode == ABPOA_LINEAR_GAP) return 0;                      /* banded linear gaps: generic kernel only (lane-exact band edges) */
-    /* RC-MSA runs on the chain (per-node read sets, poa_chain_msa_kernel); use_read_ids is what abpoa_post_set_para sets for it */
-    if ((abpt->use_read_ids && !abpt->out_msa) || abpt->out_gfa || abpt->max_n_cons > 1 || abpt->cons_algrm != ABPOA_HB) return 0;
+    /* RC-MSA and GFA run on the chain (per-node read sets, poa_chain_msa_kernel / poa_chain_gfa_kernel); use_read_ids is
+     * what abpoa_post_set_para sets for them */
+    if ((abpt->use_read_ids && !abpt->out_msa && !abpt->out_gfa) || abpt->max_n_cons > 1 || abpt->cons_algrm != ABPOA_HB) return 0;
     if (abpt->use_qv || abpt->amb_strand || abpt->inc_path_score || abpt->zdrop > 0 || abpt->rev_cigar || !abpt->ret_cigar) return 0;
     if (abpt->put_gap_on_right || abpt->put_gap_at_end) return 0;         /* handled by the kernels, but keep the chain on the common configuration */
     if (abpt->m > POA_MAX_M) return 0;
@@ -230,7 +260,7 @@ struct GroupPlan {
     size_t reads_bytes;     /* the group's part of the wave's reads region (chain_slot_reads) */
     size_t static_bytes;    /* reads_bytes + the group's own region (chain_slot_layout) */
     double pool_units_est;
-    double rec_bytes;       /* RC-MSA runs: bound on the group's result records (0 otherwise) */
+    double rec_bytes;       /* RC-MSA / GFA runs: bound on the group's result records (0 otherwise) */
 };
 
 struct Cohort {
@@ -297,7 +327,8 @@ struct ChainCall {
     bool free_run;          /* free-running schedule (default); else lock-step rounds, two kernels per round and cohort */
     int cohorts;            /* round schedule: ABPOA_GPU_CHAIN_COHORTS, or 0: as many as keep each alignment grid to one CTA per SM */
     bool want_msa; int with_cons;
-    int W;                  /* RC-MSA: words per read set (W of the largest group), 0 otherwise */
+    bool want_gfa;          /* GFA records: out_gfa with a writer attached (without one, the reference prints and computes nothing) */
+    int W;                  /* RC-MSA / GFA: words per read set (W of the largest group), 0 otherwise */
     bool export_graph;      /* the whole graph comes back (compact export) and the host computes the consensus on it */
     int sm_count;
 };
@@ -316,10 +347,11 @@ ChainCall chain_call(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_worker
     const bool serialised = launches_serialised();
     { const char *e = getenv("ABPOA_GPU_CHAIN_ROUNDS"); c.free_run = e && *e ? *e != '1' : !serialised; }
     { const char *e = getenv("ABPOA_GPU_CHAIN_EXPORT_GRAPH"); c.export_graph = e && *e == '1'; }
-    c.want_msa = abpt->out_msa != 0;
+    c.want_msa = abpt->out_msa && !abpt->out_gfa;           /* with out_gfa, abpoa_output prints only the GFA */
+    c.want_gfa = abpt->out_gfa && emit != NULL;
     c.with_cons = abpt->out_cons ? 1 : 0;
     c.W = 0;
-    if (c.want_msa) for (int g : todo) c.W = std::max(c.W, (groups[g].n_seq + 63) / 64);
+    if (c.want_msa || c.want_gfa) for (int g : todo) c.W = std::max(c.W, (groups[g].n_seq + 63) / 64);
     c.sm_count = 132;
     if (cudaDeviceGetAttribute(&c.sm_count, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || c.sm_count < 1) c.sm_count = 132;
     return c;
@@ -354,6 +386,11 @@ std::vector<GroupPlan> plan_groups(const ChainCall &c, const std::vector<int> &t
         const size_t nc = (size_t)p.n_cap;
         /* result records in the (then idle) plane pool: consensus + MSA rows, msa_len <= nodes */
         p.rec_bytes = c.want_msa ? (double)(nc + 1) * 4 + 8 + (double)(p.n_reads + c.with_cons) * (double)nc + 1024 : 0.0;
+        /* GFA: consensus + [header, ids, bases, link counts, links (a read adds at most len + 1 edges), consensus ids, read
+         * sets of the group's own words] */
+        if (c.want_gfa)
+            p.rec_bytes = (double)(nc + 1) * 4 + 4.0 * (POA_GFA_HDR_WORDS + 4 + 4.0 * (double)nc + (double)(p.bases + p.n_reads))
+                        + 8.0 * (double)nc * (double)((p.n_reads + 63) / 64) + 1024;
         /* plane units of the group's largest (last) alignment.  Free-running, a group's slab is private and its rows take
          * what their bands really need: rows 3.2 % growth per read, 2w+1 cells plus the 8-cell grid per row (5 % error,
          * 50 x 10 kbp: 25.0k rows, 29-30.4 groups per row measured; estimate 25.8k x 30).  The round schedule bump-allocates
@@ -417,7 +454,7 @@ struct Wave {
     PoaChainSync *d_sync = NULL; int32_t *d_tasks = NULL; int64_t n_tasks = 0;
     uint8_t *d_reads = NULL; size_t reads_bytes = 0;
     int32_t *d_idx = NULL; size_t idx_n = 0;                /* round index lists */
-    int64_t *d_exoff = NULL, *d_msaoff = NULL; int32_t *d_excap = NULL;
+    int64_t *d_exoff = NULL, *d_msaoff = NULL, *d_gfaoff = NULL; int32_t *d_excap = NULL;
     uint8_t *d_pool = NULL; size_t pool_bytes = 0; int32_t *d_ex = NULL;
     /* host side of the wave */
     std::vector<PoaChainSlot> hs, fin;      /* the slots as uploaded / as they came back */
@@ -431,7 +468,7 @@ struct Wave {
     int ring_rows = 2, ring_cells = 64; int gaps[4];
     /* results */
     bool cons_kernel = false; unsigned long long rec_base = 0, cons_words = 0;
-    std::vector<int64_t> recoff, msaoff, words, hoff2; int64_t tot_words = 0;
+    std::vector<int64_t> recoff, msaoff, gfaoff, words, hoff2; int64_t tot_words = 0;
     std::vector<std::vector<int32_t>> rs, rn; std::vector<std::vector<uint64_t>> rh;
     int n_failed = 0;
     /* accounting */
@@ -536,6 +573,7 @@ struct Wave {
         }
         d_exoff = (int64_t *)dtake((size_t)nw * 8); d_excap = (int32_t *)dtake((size_t)nw * 4);
         d_msaoff = c.want_msa ? (int64_t *)dtake((size_t)nw * 8) : NULL;          /* MSA record offsets */
+        d_gfaoff = c.want_gfa ? (int64_t *)dtake((size_t)nw * 8) : NULL;          /* GFA record offsets */
         /* the export buffer and the plane pool share what is left: planes are dead when the export runs */
         doff = al256(doff);
         if (doff > total) poa_die("libabpoa_b200/chain", "wave layout (%zu bytes) exceeds the arena (%zu bytes)", doff, total);
@@ -677,26 +715,36 @@ struct Wave {
     /* Join the cohort streams, run the result kernels and copy back what the host needs; the arena borrow ends here.
      * Default: heaviest-bundling consensus on the device, only consensus bytes come back.  export_graph: the whole graph
      * comes back (compact export) and the host layer computes the consensus on it -- the cross-check of the device graph
-     * against the host code.  RC-MSA: the rows are always the device's (poa_chain_msa_kernel); -r1 needs no consensus. */
+     * against the host code.  RC-MSA: the rows are always the device's (poa_chain_msa_kernel); -r1 needs no consensus.
+     * GFA: the record is always the device's (poa_chain_gfa_kernel); -r3 needs no consensus, and without a writer neither
+     * kernel runs. */
     void collect() {
         for (size_t k = 0; k < coh.size(); ++k) CK(cudaEventRecord(coh[k].ev_end, coh[k].st));
         t_enqueued = now_ms();
         for (size_t k = 1; k < coh.size(); ++k) CK(cudaStreamWaitEvent(s0, coh[k].ev_end, 0));
         CK(cudaEventRecord(ev_t1, s0));
-        const bool export_graph = c.export_graph, want_msa = c.want_msa;
+        const bool export_graph = c.export_graph, want_msa = c.want_msa, want_gfa = c.want_gfa;
         unsigned long long *d_ccur = d_cursors;               /* the pool cursors are idle now: reuse the first as the record cursor */
         int64_t *d_recoff = d_exoff;                          /* and the export offsets as record offsets */
-        /* the MSA records share the consensus records' cursor, behind the export records when the graph comes back too */
-        cons_kernel = !export_graph && (!want_msa || c.with_cons);
+        /* the MSA / GFA records share the consensus records' cursor, behind the export records when the graph comes back too */
+        if (c.abpt->out_gfa) cons_kernel = !export_graph && want_gfa && c.with_cons;
+        else cons_kernel = !export_graph && (!want_msa || c.with_cons);
+        const bool any_rec = cons_kernel || want_msa || want_gfa;
         rec_base = export_graph ? (unsigned long long)ex_words : 0;
         if (export_graph) poa_chain_export_kernel<<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw, d_ex, d_exoff, d_excap);
-        if (!export_graph || want_msa) CK(cudaMemsetAsync(d_ccur, 0, sizeof(unsigned long long), s0));
+        if (any_rec) CK(cudaMemsetAsync(d_ccur, 0, sizeof(unsigned long long), s0));
         if (cons_kernel) poa_chain_consensus_kernel<<<nw, 32, 0, s0>>>(d_slots, d_cp, nw, d_ex, d_ccur, (unsigned long long)(pool_bytes / 4), d_recoff);
         CK(cudaGetLastError());
         launches += (export_graph || cons_kernel) ? 1 : 0;
         if (want_msa) {
             poa_chain_msa_kernel<<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw, c.with_cons, export_graph && c.with_cons, d_ex, d_ccur, rec_base,
                                                             (unsigned long long)(pool_bytes / 4), d_msaoff);
+            CK(cudaGetLastError());
+            ++launches;
+        }
+        if (want_gfa) {
+            poa_chain_gfa_kernel<<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw, c.with_cons, export_graph && c.with_cons, d_ex, d_ccur, rec_base,
+                                                            (unsigned long long)(pool_bytes / 4), d_gfaoff);
             CK(cudaGetLastError());
             ++launches;
         }
@@ -714,16 +762,18 @@ struct Wave {
         }
         t_dev_done = now_ms();
         /* device results: record offsets, then one copy of all records */
-        recoff.assign((size_t)nw, -1); msaoff.assign((size_t)nw, -1);
-        if (!export_graph || want_msa) {           /* records: [rec_base, rec_base + cursor) words of d_ex */
-            int64_t *h_ro = NULL; CK(cudaHostAlloc((void **)&h_ro, (size_t)nw * 16 + 8, cudaHostAllocDefault));
+        recoff.assign((size_t)nw, -1); msaoff.assign((size_t)nw, -1); gfaoff.assign((size_t)nw, -1);
+        if (any_rec) {                             /* records: [rec_base, rec_base + cursor) words of d_ex */
+            int64_t *h_ro = NULL; CK(cudaHostAlloc((void **)&h_ro, (size_t)nw * 24 + 8, cudaHostAllocDefault));
             if (cons_kernel) CK(cudaMemcpyAsync(h_ro, d_recoff, (size_t)nw * 8, cudaMemcpyDeviceToHost, s0));
             if (want_msa) CK(cudaMemcpyAsync(h_ro + nw, d_msaoff, (size_t)nw * 8, cudaMemcpyDeviceToHost, s0));
-            CK(cudaMemcpyAsync(h_ro + 2 * nw, d_ccur, 8, cudaMemcpyDeviceToHost, s0));
+            if (want_gfa) CK(cudaMemcpyAsync(h_ro + 2 * nw, d_gfaoff, (size_t)nw * 8, cudaMemcpyDeviceToHost, s0));
+            CK(cudaMemcpyAsync(h_ro + 3 * nw, d_ccur, 8, cudaMemcpyDeviceToHost, s0));
             CK(cudaStreamSynchronize(s0));
             if (cons_kernel) memcpy(recoff.data(), h_ro, (size_t)nw * 8);
             if (want_msa) memcpy(msaoff.data(), h_ro + nw, (size_t)nw * 8);
-            cons_words = (unsigned long long)h_ro[2 * nw];
+            if (want_gfa) memcpy(gfaoff.data(), h_ro + 2 * nw, (size_t)nw * 8);
+            cons_words = (unsigned long long)h_ro[3 * nw];
             CK(cudaFreeHost(h_ro));
             if (rec_base + cons_words > pool_bytes / 4) cons_words = pool_bytes / 4 - rec_base;
             h_cons = (int32_t *)pinned_get(2, (size_t)std::max<unsigned long long>(cons_words, 1) * 4);
@@ -740,7 +790,7 @@ struct Wave {
         }
         words.assign((size_t)nw, 0); hoff2.assign((size_t)nw, 0);
         for (int t = 0; t < nw; ++t) {
-            const bool rec_ok = (!cons_kernel || recoff[t] >= 0) && (!want_msa || msaoff[t] >= 0);
+            const bool rec_ok = (!cons_kernel || recoff[t] >= 0) && (!want_msa || msaoff[t] >= 0) && (!want_gfa || gfaoff[t] >= 0);
             if (!export_graph) { words[t] = (!fin[t].failed && rec_ok) ? 1 : 0; continue; }
             if (fin[t].failed || hdr4[4 * t] < 2 || !rec_ok) continue;
             words[t] = 4 + 5ll * hdr4[4 * t] + 4ll * hdr4[4 * t + 1] + hdr4[4 * t + 2];
@@ -800,7 +850,9 @@ struct Wave {
                         const int32_t *rec = h_cons + (msaoff[t] - (int64_t)rec_base);
                         poa_msa_install(ab, p.n_reads, rec[1], rec[0], reinterpret_cast<const uint8_t *>(rec + 2));
                     }
+                    if (c.want_gfa) poa_gfa_install(ab, h_cons + (gfaoff[t] - (int64_t)rec_base));     /* printed by abpoa_generate_gfa */
                     poa_finish_group_result(ab, abpt, o, c.emit, p.g);
+                    if (c.want_gfa) poa_gfa_install(ab, NULL);
                     o->dp_cells = fin[t].cells; o->n_aligned = p.n_reads - 1;
                     if (c.record) {
                         const int nr = p.n_reads;

@@ -757,4 +757,98 @@ POA_DEV void chain_msa_rows(PoaChainSlot *s, const PoaChainParams *cp, int msa_l
     POA_CTA_SYNC();
 }
 
+/* ------------------------------------------------------------------ GFA on the device
+ * The record abpoa_generate_gfa prints (layout: poa_gfa_t in poa_internal.h; text: poa_gfa_format in poa_cons.c).  The
+ * reference's writer (src/abpoa_output.c:194-294) lists the nodes in FIFO Kahn order from SRC and builds each read's path
+ * from the union of the read sets of a node's out-edges, which is the node's read set here.
+ *
+ * chain_gfa_order (host twin: gfa_describe_host): Kahn from SRC with a FIFO queue, out-edges in list order, stopping when
+ * SINK is dequeued -- not the LIFO order of chain_msa_rank.  Serial, on one thread.  Leaves the queue in scr[4] (SRC, then
+ * the segments) and returns the number of segments, or -1; *n_link = the segments' in-links from nodes other than SRC.
+ * scr[3] holds the in-degrees; scr[1] (the consensus path of chain_consensus) is left alone. */
+#define POA_GFA_HDR_WORDS 6             /* header words of a record (POA_GFA_HDR in poa_internal.h) */
+
+POA_DEV int chain_gfa_order(PoaChainSlot *s, const PoaChainParams *cp, int *n_link) {
+    if (!POA_TID0) return -1;
+    const int K = cp->K, n = s->n_nodes;
+    int32_t *deg = s->scr[3], *q = s->scr[4];
+    if (s->failed || n < 3) return -1;
+    for (int v = 0; v < n; ++v) deg[v] = s->in_cnt[v];
+    int head = 0, tail = 0, links = 0;
+    q[tail++] = 0;
+    while (head < tail) {
+        const int cur = q[head++];
+        if (cur == 1) { *n_link = links; return head - 2; }
+        if (cur != 0) {
+            const int32_t *iid = s->in_id + (size_t)cur * K;
+            for (int e = 0; e < s->in_cnt[cur]; ++e) links += iid[e] != 0;
+        }
+        const int32_t *oid = s->out_id + (size_t)cur * K;
+        for (int e = 0; e < s->out_cnt[cur]; ++e) {
+            const int v = oid[e];
+            if (--deg[v] == 0) { if (tail >= n) return -1; q[tail++] = v; }
+        }
+    }
+    return -1;
+}
+
+/* The header of a group's record (order on one thread: chain_gfa_order; with_cons: the path chain_consensus left in
+ * scr[1]) and its size in int32 words, or -1.  Read sets take the group's own ceil(n_reads / 64) words, not W. */
+POA_DEV int64_t chain_gfa_size(PoaChainSlot *s, const PoaChainParams *cp, int with_cons, int32_t *hdr) {
+    int n_link = 0;
+    const int n_seg = chain_gfa_order(s, cp, &n_link);
+    if (n_seg < 0) return -1;
+    const int n = s->n_nodes, words = (s->n_reads + 63) / 64;
+    int nl = -s->out_cnt[0];
+    for (int v = 2; v < n; ++v) nl += s->in_cnt[v];
+    int cons_len = -1;
+    if (with_cons) {
+        const int32_t *nxt = s->scr[1];
+        cons_len = 0;
+        for (int cur = nxt[0]; cur != 1 && cur >= 0; cur = nxt[cur]) if (++cons_len > n) return -1;
+    }
+    hdr[0] = n_seg; hdr[1] = n_link; hdr[2] = n - 2; hdr[3] = nl; hdr[4] = words; hdr[5] = cons_len;
+    int64_t w = POA_GFA_HDR_WORDS + 3ll * n_seg + n_link + (cons_len > 0 ? cons_len : 0);
+    return (w + 1) / 2 * 2 + 2ll * n_seg * words;
+}
+
+/* The record itself (header from chain_gfa_size) at `rec`, 8-byte aligned.  Needs the whole CTA; scr[3] becomes the
+ * link offsets (the in-degrees are dead). */
+POA_DEV void chain_gfa_record(PoaChainSlot *s, const PoaChainParams *cp, const int32_t *hdr, int32_t *rec) {
+    const int K = cp->K, W = cp->W;
+    const int n_seg = hdr[0], n_link = hdr[1], words = hdr[4], cons_len = hdr[5];
+    const int32_t *q = s->scr[4] + 1, *nxt = s->scr[1];
+    int32_t *lo = s->scr[3];
+    int32_t *seg_id = rec + POA_GFA_HDR_WORDS, *seg_base = seg_id + n_seg, *link_cnt = seg_base + n_seg, *link_from = link_cnt + n_seg;
+    int32_t *cons_id = link_from + n_link;
+    const int64_t w = POA_GFA_HDR_WORDS + 3ll * n_seg + n_link + (cons_len > 0 ? cons_len : 0);
+    uint64_t *sets = reinterpret_cast<uint64_t *>(rec + (w + 1) / 2 * 2);
+    if (POA_TID0) for (int k = 0; k < POA_GFA_HDR_WORDS; ++k) rec[k] = hdr[k];
+    POA_PAR_FOR(i, n_seg) {
+        const int v = q[i];
+        const int32_t *iid = s->in_id + (size_t)v * K;
+        int c = 0;
+        for (int e = 0; e < s->in_cnt[v]; ++e) c += iid[e] != 0;
+        seg_id[i] = v; seg_base[i] = s->base[v]; link_cnt[i] = c; lo[i] = c;
+    }
+    POA_CTA_SYNC();
+    cta_excl_scan(lo, n_seg);
+    POA_CTA_SYNC();
+    POA_PAR_FOR(i, n_seg) {
+        const int v = q[i];
+        const int32_t *iid = s->in_id + (size_t)v * K;
+        int32_t *to = link_from + lo[i];
+        for (int e = 0; e < s->in_cnt[v]; ++e) if (iid[e] != 0) *to++ = iid[e];
+    }
+    POA_PAR_FOR(k, n_seg * words) {
+        const int i = k / words, wd = k - i * words;
+        sets[k] = s->read_set[(size_t)q[i] * W + wd];
+    }
+    if (cons_len > 0 && POA_TID0) {
+        int j = 0;
+        for (int cur = nxt[0]; cur != 1 && cur >= 0 && j < cons_len; cur = nxt[cur]) cons_id[j++] = cur;
+    }
+    POA_CTA_SYNC();
+}
+
 #endif

@@ -7,9 +7,10 @@
  *   phred of a column   reference src/abpoa_output.c:296-302
  *   RC-MSA              reference src/abpoa_output.c:105-192
  *   writers             reference src/abpoa_output.c:72-103, :588-627
+ *   GFA                 reference src/abpoa_output.c:194-294
  *   abpoa_output        reference src/abpoa_align.c:354-370
  * Out of the hot-path scope and therefore not provided (they abort with a message):
- * most-frequent-base consensus, multi-consensus clustering (max_n_cons > 1), GFA, dot.
+ * most-frequent-base consensus, multi-consensus clustering (max_n_cons > 1), dot.
  */
 #include <math.h>
 #include "poa_internal.h"
@@ -232,9 +233,191 @@ void abpoa_output_rc_msa(abpoa_t *ab, abpoa_para_t *abpt, FILE *out_fp) {
         }
 }
 
+/* ------------------------------------------------------------------ GFA
+ * H line, then per segment in FIFO Kahn order from SRC (stopping at SINK) its S line and one L line per in-link, then one
+ * P line per read (its segments in that order; reads with is_rc reversed, with '-') and with -r 4 the consensus path.  A
+ * path with no segment prints "P\t<name>\t" and nothing else, as the reference does.  A headline group has ~500 k path
+ * entries: numbers go through put_int into one buffer, not through stdio. */
+typedef struct { char *s; size_t l, m; } gfa_buf;
+
+static inline void gb_need(gfa_buf *b, size_t n) {
+    if (b->l + n <= b->m) return;
+    b->m = (b->l + n) * 2 + 4096;
+    b->s = (char *)poa_xrealloc(b->s, b->m);
+}
+static inline void put_str(gfa_buf *b, const char *s, size_t n) { gb_need(b, n); memcpy(b->s + b->l, s, n); b->l += n; }
+#define PUT_LIT(b, lit) put_str((b), (lit), sizeof(lit) - 1)
+static inline void put_int(gfa_buf *b, int v) {
+    char t[12]; int k = 0;
+    unsigned u = v < 0 ? 0u - (unsigned)v : (unsigned)v;
+    do { t[k++] = (char)('0' + u % 10); u /= 10; } while (u);
+    gb_need(b, 12);
+    if (v < 0) b->s[b->l++] = '-';
+    while (k) b->s[b->l++] = t[--k];
+}
+
+void poa_gfa_from_record(poa_gfa_t *g, const int32_t *rec) {
+    g->n_seg = rec[0]; g->n_link = rec[1]; g->ns = rec[2]; g->nl = rec[3]; g->words = rec[4]; g->cons_len = rec[5];
+    const int32_t *p = rec + POA_GFA_HDR;
+    g->seg_id = p; p += g->n_seg;
+    g->seg_base = p; p += g->n_seg;
+    g->link_cnt = p; p += g->n_seg;
+    g->link_from = p; p += g->n_link;
+    g->cons_id = p; p += POA_MAX(g->cons_len, 0);
+    if ((p - rec) & 1) ++p;
+    g->read_set = (const uint64_t *)(const void *)p;
+}
+
+char *poa_gfa_format(const poa_gfa_t *g, const abpoa_seq_t *abs, int np, size_t *len) {
+    gfa_buf b = { NULL, 0, 0 };
+    const int n_seq = abs->n_seq;
+    PUT_LIT(&b, "H\tVN:Z:1.0\tNS:i:"); put_int(&b, g->ns); PUT_LIT(&b, "\tNL:i:"); put_int(&b, g->nl);
+    PUT_LIT(&b, "\tNP:i:"); put_int(&b, np); PUT_LIT(&b, "\n");
+    for (int i = 0, k = 0; i < g->n_seg; ++i) {
+        const int id = g->seg_id[i] - 1;
+        PUT_LIT(&b, "S\t"); put_int(&b, id); gb_need(&b, 3);
+        b.s[b.l++] = '\t'; b.s[b.l++] = ab_char256_table[g->seg_base[i]]; b.s[b.l++] = '\n';
+        for (int e = 0; e < g->link_cnt[i]; ++e, ++k) {
+            PUT_LIT(&b, "L\t"); put_int(&b, g->link_from[k] - 1); PUT_LIT(&b, "\t+\t"); put_int(&b, id); PUT_LIT(&b, "\t+\t0M\n");
+        }
+    }
+    /* read sets -> paths: count, then place every segment into the paths of its reads, in segment order */
+    int64_t *off = (int64_t *)poa_xcalloc((size_t)n_seq + 1, sizeof(int64_t));
+    for (int i = 0; i < g->n_seg; ++i)
+        for (int wd = 0; wd < g->words; ++wd)
+            for (uint64_t bits = g->read_set[(size_t)i * g->words + wd]; bits; bits &= bits - 1) {
+                const int r = wd * 64 + __builtin_ctzll(bits);
+                if (r < n_seq) ++off[r + 1];
+            }
+    for (int r = 0; r < n_seq; ++r) off[r + 1] += off[r];
+    int32_t *path = (int32_t *)poa_xmalloc((size_t)POA_MAX(off[n_seq], 1) * sizeof(int32_t));
+    int64_t *fill = (int64_t *)poa_xmalloc((size_t)POA_MAX(n_seq, 1) * sizeof(int64_t));
+    memcpy(fill, off, (size_t)n_seq * sizeof(int64_t));
+    for (int i = 0; i < g->n_seg; ++i)
+        for (int wd = 0; wd < g->words; ++wd)
+            for (uint64_t bits = g->read_set[(size_t)i * g->words + wd]; bits; bits &= bits - 1) {
+                const int r = wd * 64 + __builtin_ctzll(bits);
+                if (r < n_seq) path[fill[r]++] = g->seg_id[i] - 1;
+            }
+    for (int r = 0; r < n_seq; ++r) {
+        PUT_LIT(&b, "P\t");
+        if (abs->name[r].l > 0) put_str(&b, abs->name[r].s, (size_t)abs->name[r].l); else put_int(&b, r + 1);
+        PUT_LIT(&b, "\t");
+        const int32_t *p = path + off[r];
+        const int64_t n = off[r + 1] - off[r];
+        const int rc = abs->is_rc[r];
+        for (int64_t j = 0; j < n; ++j) {
+            if (j) PUT_LIT(&b, ",");
+            put_int(&b, p[rc ? n - 1 - j : j]);
+            gb_need(&b, 1); b.s[b.l++] = rc ? '-' : '+';
+        }
+        if (n > 0) PUT_LIT(&b, "\t*\n");
+    }
+    if (g->cons_len >= 0) {
+        PUT_LIT(&b, "P\tConsensus_sequence\t");
+        for (int j = 0; j < g->cons_len; ++j) {
+            if (j) PUT_LIT(&b, ",");
+            put_int(&b, g->cons_id[j] - 1); PUT_LIT(&b, "+");
+        }
+        if (g->cons_len > 0) PUT_LIT(&b, "\t*\n");
+    }
+    free(off); free(path); free(fill);
+    *len = b.l;
+    return b.s;
+}
+
+/* the description of the host graph (per-edge read sets); arrays in *store, released with free() */
+typedef struct { int32_t *ints; uint64_t *sets; } gfa_store;
+
+static void gfa_describe_host(abpoa_t *ab, abpoa_para_t *abpt, poa_gfa_t *g, gfa_store *st) {
+    const abpoa_graph_t *abg = ab->abg;
+    const abpoa_node_t *node = abg->node;
+    const int n = abg->node_n, n_seq = ab->abs->n_seq, words = (n_seq + 63) / 64;
+    int64_t n_in = 0;
+    for (int v = 0; v < n; ++v) n_in += node[v].in_edge_n;
+    /* q | deg | seg_base | link_cnt | link_from | cons_id */
+    int32_t *q = (int32_t *)poa_xmalloc(((size_t)5 * n + (size_t)n_in + 1) * sizeof(int32_t));
+    int32_t *deg = q + n, *seg_base = deg + n, *link_cnt = seg_base + n, *cons_id = link_cnt + n, *link_from = cons_id + n;
+    for (int v = 0; v < n; ++v) deg[v] = node[v].in_edge_n;
+    int head = 0, tail = 0, n_link = 0;
+    q[tail++] = ABPOA_SRC_NODE_ID;
+    while (head < tail) {
+        const int cur = q[head++];
+        if (cur == ABPOA_SINK_NODE_ID) break;
+        if (cur != ABPOA_SRC_NODE_ID) {
+            const int i = head - 2;
+            seg_base[i] = node[cur].base; link_cnt[i] = 0;
+            for (int e = 0; e < node[cur].in_edge_n; ++e)
+                if (node[cur].in_id[e] != ABPOA_SRC_NODE_ID) { link_from[n_link++] = node[cur].in_id[e]; ++link_cnt[i]; }
+        }
+        for (int e = 0; e < node[cur].out_edge_n; ++e)
+            if (--deg[node[cur].out_id[e]] == 0) q[tail++] = node[cur].out_id[e];
+    }
+    g->n_seg = q[head - 1] == ABPOA_SINK_NODE_ID ? head - 2 : head - 1;
+    g->n_link = n_link; g->ns = n - 2; g->words = words;
+    int nl = 0;
+    for (int v = 2; v < n; ++v) nl += node[v].in_edge_n;
+    g->nl = nl - node[ABPOA_SRC_NODE_ID].out_edge_n;
+    g->seg_id = q + 1; g->seg_base = seg_base; g->link_cnt = link_cnt; g->link_from = link_from;
+    /* a read passes through a node iff one of the node's out-edges carries it */
+    uint64_t *sets = (uint64_t *)poa_xcalloc((size_t)POA_MAX(g->n_seg, 1) * POA_MAX(words, 1), sizeof(uint64_t));
+    for (int i = 0; i < g->n_seg; ++i) {
+        const abpoa_node_t *nd = &node[q[1 + i]];
+        const int nw = POA_MIN(nd->read_ids_n, words);
+        for (int e = 0; e < nd->out_edge_n; ++e)
+            for (int wd = 0; wd < nw; ++wd) sets[(size_t)i * words + wd] |= nd->read_ids[e][wd];
+    }
+    g->read_set = sets;
+    g->cons_len = -1; g->cons_id = cons_id;
+    if (abpt->out_cons) {
+        abpoa_generate_consensus(ab, abpt);
+        const abpoa_cons_t *abc = ab->abc;
+        g->cons_len = 0;
+        if (abc->n_cons > 0) {
+            g->cons_len = abc->cons_len[0];
+            memcpy(cons_id, abc->cons_node_ids[0], (size_t)g->cons_len * sizeof(int32_t));
+        }
+    }
+    st->ints = q; st->sets = sets;
+}
+
+/* FIFO order of the host writer (tests compare the device's with it): segment ids into out, returns their number */
+int poa_gfa_host_order(abpoa_t *ab, int32_t *out) {
+    abpoa_para_t para; memset(&para, 0, sizeof para);       /* out_cons = 0: no consensus */
+    poa_graph_sync_public(ab->abg);
+    poa_gfa_t g; gfa_store st;
+    gfa_describe_host(ab, &para, &g, &st);
+    memcpy(out, g.seg_id, (size_t)g.n_seg * sizeof(int32_t));
+    free(st.ints); free(st.sets);
+    return g.n_seg;
+}
+
+void poa_gfa_install(abpoa_t *ab, const int32_t *rec) { poa_graph_set_gfa_record(ab->abg, rec); }
+
+/* A record text as abpoa_generate_gfa prints it (for tests: the device record through the product's formatter) */
+char *poa_gfa_record_text(const int32_t *rec, abpoa_t *ab, abpoa_para_t *abpt, size_t *len) {
+    poa_gfa_t g; poa_gfa_from_record(&g, rec);
+    return poa_gfa_format(&g, ab->abs, ab->abs->n_seq + abpt->out_cons, len);
+}
+
 void abpoa_generate_gfa(abpoa_t *ab, abpoa_para_t *abpt, FILE *out_fp) {
-    (void)ab; (void)abpt; (void)out_fp;
-    poa_die(__func__, "GFA output is outside the scope of the GPU hot-path library.");
+    if (!out_fp) return;                                   /* nothing printed, nothing computed */
+    abpoa_graph_t *abg = ab->abg;
+    poa_graph_sync_public(abg);
+    const int32_t *rec = poa_graph_gfa_record(abg);
+    poa_gfa_t g; gfa_store st = { NULL, NULL };
+    if (rec) {
+        poa_gfa_from_record(&g, rec);
+        /* the consensus fields: installed with the record (poa_cons_install), or computed on an imported graph */
+        if (abpt->out_cons) abpoa_generate_consensus(ab, abpt);
+    } else {
+        if (abg->node_n <= 2) return;
+        gfa_describe_host(ab, abpt, &g, &st);
+    }
+    size_t len = 0;
+    char *text = poa_gfa_format(&g, ab->abs, ab->abs->n_seq + abpt->out_cons, &len);
+    fwrite(text, 1, len, out_fp);
+    free(text); free(st.ints); free(st.sets);
 }
 
 void abpoa_dump_pog(abpoa_t *ab, abpoa_para_t *abpt) {

@@ -53,6 +53,7 @@ typedef struct {
     int public_stale;                           /* node[].n_read / n_span_read lag behind the dense arrays */
     int has_read_ids;                           /* some out-edge carries a read-id bitset */
     int msa_installed;                          /* abc holds RC-MSA rows computed elsewhere (poa_msa_install) for this graph */
+    const int32_t *gfa_rec;                     /* borrowed GFA record computed elsewhere (poa_gfa_install), or NULL */
     int *touched; int n_touched, touched_m; uint8_t *touch_mark;   /* nodes whose edge lists changed since the last ordering */
     int64_t n_edges;                            /* total in-edges in the graph        */
     /* nodes the Kahn passes must COUNT for: in-degree >= 2 or member of an aligned group (forward
@@ -277,7 +278,7 @@ void abpoa_reset(abpoa_t *ab, abpoa_para_t *abpt, int qlen) {
         memset(x->cin, 0, (size_t)abg->node_n * sizeof(int)); memset(x->cout, 0, (size_t)abg->node_n * sizeof(int));
         memset(x->caln, 0, (size_t)abg->node_n * sizeof(int));
         memset(x->cnread, 0, (size_t)abg->node_n * sizeof(int)); memset(x->cspan, 0, (size_t)abg->node_n * sizeof(int));
-        x->span_pending = 0; x->public_stale = 0; x->has_read_ids = 0; x->msa_installed = 0;
+        x->span_pending = 0; x->public_stale = 0; x->has_read_ids = 0; x->msa_installed = 0; x->gfa_rec = NULL;
         for (int t = 0; t < x->n_touched; ++t) x->touch_mark[x->touched[t]] = 0;
         x->n_touched = 0; x->n_edges = 0;
         for (int t = 0; t < x->n_fwd; ++t) x->fwd_mark[x->fwd_list[t]] = 0;
@@ -766,7 +767,7 @@ static void seed_graph_with_sequence(abpoa_graph_t *abg, abpoa_para_t *abpt, con
         last = cur;
     }
     edge_add(abg, last, ABPOA_SINK_NODE_ID, 0, weight[seq_l - 1], add_read_id, add_read_weight, read_id, read_ids_n, tot_read_n);
-    abg->is_called_cons = abg->is_set_msa_rank = abg->is_topological_sorted = 0; gx(abg)->msa_installed = 0;
+    abg->is_called_cons = abg->is_set_msa_rank = abg->is_topological_sorted = 0; gx(abg)->msa_installed = 0; gx(abg)->gfa_rec = NULL;
     abpoa_topological_sort(abg, abpt);
     bump_span_reads(abg, ABPOA_SRC_NODE_ID, ABPOA_SINK_NODE_ID, 1);
 }
@@ -857,7 +858,7 @@ int poa_add_alignment_nosync(abpoa_t *ab, abpoa_para_t *abpt, int beg_node_id, i
             } /* ABPOA_CDEL: the read skips this node */
         }
         edge_add(abg, last_id, end_node_id, 1 - last_is_new, weight[seq_l - 1], add_read_id, add_read_weight, read_id, read_ids_n, tot_read_n);
-        abg->is_called_cons = abg->is_set_msa_rank = abg->is_topological_sorted = 0; x->msa_installed = 0;
+        abg->is_called_cons = abg->is_set_msa_rank = abg->is_topological_sorted = 0; x->msa_installed = 0; x->gfa_rec = NULL;
         poa_prof_ms[3] += prof_now() - tf0;
         abpoa_topological_sort(abg, abpt);
         const double tf1 = prof_now();
@@ -919,13 +920,15 @@ void poa_graph_import(abpoa_t *ab, abpoa_para_t *abpt, const int32_t *ex) {
         x->cnread[v] = n_read[v]; x->cspan[v] = n_fused;
     }
     if (pi != n_in || po != n_in) poa_die(__func__, "inconsistent export: %d in-edges, %d out-edges, header says %d", pi, po, n_in);
-    x->n_edges = n_in; x->public_stale = 1; x->span_pending = 0; x->msa_installed = 0;
+    x->n_edges = n_in; x->public_stale = 1; x->span_pending = 0; x->msa_installed = 0; x->gfa_rec = NULL;
     abg->is_topological_sorted = abg->is_called_cons = abg->is_set_msa_rank = 0;
     poa_graph_sync_public(abg);
 }
 
 int poa_graph_msa_installed(const abpoa_graph_t *abg) { return cgx(abg)->msa_installed; }
 void poa_graph_set_msa_installed(abpoa_graph_t *abg) { gx(abg)->msa_installed = 1; }
+const int32_t *poa_graph_gfa_record(const abpoa_graph_t *abg) { return cgx(abg)->gfa_rec; }
+void poa_graph_set_gfa_record(abpoa_graph_t *abg, const int32_t *rec) { gx(abg)->gfa_rec = rec; }
 
 /* ------------------------------------------------------------------ sub-graph windows
  * abpoa_subgraph_nodes (reference src/abpoa_graph.c:595-687): widen the index window

@@ -57,6 +57,31 @@ void poa_cons_install(abpoa_t *ab, int n_seq, int len, const uint8_t *base, cons
 void poa_msa_install(abpoa_t *ab, int n_seq, int n_rows, int msa_len, const uint8_t *rows);
 int poa_graph_msa_installed(const abpoa_graph_t *abg);  /* abc holds installed rows for the current graph */
 void poa_graph_set_msa_installed(abpoa_graph_t *abg);
+/* GFA (-r 3 / -r 4).  One formatter prints every GFA this library writes, from a compact description of the graph:
+ * the segments (node ids >= 2) in the writer's FIFO Kahn order, the base and in-links of each (SRC excluded, in in-edge
+ * order), the set of reads whose path passes through each, and optionally the consensus path.  The host graph
+ * (abpoa_generate_gfa) and the device chain's record (poa_chain.cuh: chain_gfa_record) both feed it.
+ * A record is int32 words, its start 8-byte aligned:
+ *   [0] n_seg  [1] n_link  [2] NS (node_n - 2)  [3] NL  [4] words per read set  [5] consensus length, -1: none
+ *   seg_id[n_seg], seg_base[n_seg], link_cnt[n_seg], link_from[n_link], cons_id[max(0, cons_len)], one pad word if
+ *   the count so far is odd, then the read sets as uint64 [n_seg][words] */
+typedef struct {
+    int n_seg, n_link, ns, nl, words, cons_len;
+    const int32_t *seg_id, *seg_base, *link_cnt, *link_from, *cons_id;
+    const uint64_t *read_set;
+} poa_gfa_t;
+#define POA_GFA_HDR 6
+void poa_gfa_from_record(poa_gfa_t *g, const int32_t *rec);
+/* the text for the reads of `abs` (names, is_rc); np = the header's NP; returns a malloc'ed buffer of *len bytes */
+char *poa_gfa_format(const poa_gfa_t *g, const abpoa_seq_t *abs, int np, size_t *len);
+/* a GFA record computed elsewhere (the device chain) for the handle's current group: abpoa_generate_gfa prints it
+ * instead of walking the host graph.  Borrowed: install NULL before the record's memory goes away. */
+void poa_gfa_install(abpoa_t *ab, const int32_t *rec);
+/* for the tests: the host writer's segment order (returns n_seg), and a record's text as abpoa_generate_gfa prints it */
+int poa_gfa_host_order(abpoa_t *ab, int32_t *out);
+char *poa_gfa_record_text(const int32_t *rec, abpoa_t *ab, abpoa_para_t *abpt, size_t *len);
+const int32_t *poa_graph_gfa_record(const abpoa_graph_t *abg);
+void poa_graph_set_gfa_record(abpoa_graph_t *abg, const int32_t *rec);
 int poa_edge_path_score(const abpoa_graph_t *abg, int node_id, int in_idx);  /* -G scores */
 /* dense, node-id-indexed views kept by poa_graph.c (see poa_graph_x) */
 void poa_graph_sync_public(abpoa_graph_t *abg);        /* fold dense n_read / n_span_read into node[] */

@@ -14,10 +14,10 @@
  *
  * Two engines sit behind abpoa_gpu_msa_batch (DESIGN.md section 5).  The device-resident CHAIN engine keeps
  * the graph of every group in HBM and runs align -> fuse -> re-order -> flatten entirely on the GPU (global,
- * banded, consensus and/or RC-MSA output): two persistent kernels per batch -- one resident warp per group
+ * banded, consensus, RC-MSA or GFA output): two persistent kernels per batch -- one resident warp per group
  * running its alignments back to back, one fuse CTA per SM serving a task queue -- so every group advances at
- * its own pace; reads go up once, consensus bytes and MSA rows come back once.  Everything else -- local /
- * extend mode, GFA, -d > 1, -a 1, -s, -G, quality weights, groups that outgrow their device slot -- runs on the
+ * its own pace; reads go up once, consensus bytes, MSA rows and GFA records come back once.  Everything else --
+ * local / extend mode, -d > 1, -a 1, -s, -G, quality weights, groups that outgrow their device slot -- runs on the
  * LAUNCH engine: worker threads flatten and fuse on the host and launch one kernel grid per round, each
  * worker keeping ABPOA_GPU_PIPE_DEPTH sub-chunks in flight.  Same results either way.
  */
@@ -89,7 +89,7 @@ int abpoa_gpu_msa_batch(abpoa_gpu_batch_t *eng, abpoa_para_t *abpt, int n_groups
 void abpoa_gpu_group_result_free(abpoa_gpu_group_result_t *r);
 
 /* The same, plus the text `abpoa -l` prints: for every group, in group order, what abpoa_output() writes
- * (consensus FASTA / FASTQ or RC-MSA according to abpt, consensus headers numbered by group as the reference
+ * (consensus FASTA / FASTQ, RC-MSA or GFA according to abpt, consensus headers numbered by group as the reference
  * CLI does in list mode, src/abpoa.c:148-168).  names[g][i]: name of read i of group g (names or names[g]
  * may be NULL: rows are called Seq_1 ...).  results may be NULL. */
 int abpoa_gpu_msa_batch_write(abpoa_gpu_batch_t *eng, abpoa_para_t *abpt, int n_groups, const abpoa_gpu_group_t *groups,
