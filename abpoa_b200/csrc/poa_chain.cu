@@ -15,7 +15,7 @@
  *                              and under tools that serialise kernel launches (profilers, sanitizers), where two kernels
  *                              that wait for each other cannot both run.
  *
- * The results come from the device: poa_chain_consensus_kernel (heaviest bundling), poa_chain_msa_kernel (row-column
+ * The results come from the device: poa_chain_consensus_kernel (heaviest bundling or most frequent base), poa_chain_msa_kernel (row-column
  * MSA) and poa_chain_gfa_kernel (GFA) write records that come back in one copy and are installed into the caller's records.  With
  * ABPOA_GPU_CHAIN_EXPORT_GRAPH=1 the whole graph comes back instead (poa_chain_export_kernel, rebuilt by
  * poa_graph_import) and the host computes the consensus on it: the cross-check of the device graph against the host
@@ -26,9 +26,9 @@
  * that fit the arena (split_waves) and runs each wave (Wave).  A group's device region is laid out by chain_slot_layout
  * (poa_chain.cuh) for the planner and the carve alike.
  *
- * Scope of the chain: global alignment, banded (wb >= 0), packed-int16 admissible scores, heaviest-bundling
- * consensus, row-column MSA and GFA (one read set per node, not per edge), unit base weights.  Everything else
- * takes the other engine.
+ * Scope of the chain: global alignment, banded (wb >= 0), packed-int16 admissible scores, heaviest-bundling or
+ * most-frequent-base consensus (single cluster, no sub_aln), row-column MSA and GFA (one read set per node, not per
+ * edge), unit base weights.  Everything else takes the other engine.
  */
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -154,14 +154,16 @@ __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_export_kernel(PoaChainS
     }
 }
 
-/* consensus of every finished group (chain_consensus: heaviest bundling on one thread per group); records are packed
- * back to back into `out` through an atomic cursor: rec_off[g] = first word of group g's record, -1 if none */
-__global__ void __launch_bounds__(32) poa_chain_consensus_kernel(PoaChainSlot *slots, const PoaChainParams *cp, int n,
-                                                                 int32_t *out, unsigned long long *cursor, unsigned long long out_words, int64_t *rec_off) {
-    if ((int)blockIdx.x >= n || threadIdx.x != 0) return;
+/* consensus of every finished group (chain_cons_path: heaviest bundling on one thread per group, most frequent base on a
+ * CTA per group: launched with 32 or POA_CHAIN_T threads); records are packed back to back into `out` through an atomic cursor:
+ * rec_off[g] = first word of group g's record, -1 if none */
+__global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_consensus_kernel(PoaChainSlot *slots, const PoaChainParams *cp, int n,
+                                                                          int32_t *out, unsigned long long *cursor, unsigned long long out_words, int64_t *rec_off) {
+    if ((int)blockIdx.x >= n) return;
     PoaChainSlot *s = &slots[blockIdx.x];
     int32_t *tmp = s->scr[2];                               /* [n_cap]: the consensus is never longer than the graph */
-    chain_consensus(s, cp, tmp, s->n_cap);
+    chain_cons_path(s, cp, tmp, s->n_cap);
+    if (threadIdx.x != 0) return;
     const int len = tmp[0];
     if (len < 0) { rec_off[blockIdx.x] = -1; return; }
     const unsigned long long at = atomicAdd(cursor, (unsigned long long)(len + 1));
@@ -171,7 +173,7 @@ __global__ void __launch_bounds__(32) poa_chain_consensus_kernel(PoaChainSlot *s
 }
 
 /* RC-MSA of every finished group, one CTA per group: ranks on one thread (chain_msa_rank), rows by the whole CTA
- * (chain_msa_rows).  with_cons: add the consensus row, from the path chain_consensus left in scr[1] -- run_cons: compute
+ * (chain_msa_rows).  with_cons: add the consensus row, from the path chain_cons_path left in scr[1] -- run_cons: compute
  * that path here (the consensus kernel did not run).  A record is [msa_len, n_rows, rows as bytes], packed through the
  * same cursor as the consensus records, at word rec_base + cursor; rec_off[g] = -1 if the group has none (it is then
  * finished by the launch engine). */
@@ -182,8 +184,8 @@ __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_msa_kernel(PoaChainSlot
     __shared__ long long at_s;
     __shared__ int len_s;
     PoaChainSlot *s = &slots[blockIdx.x];
+    if (run_cons && !s->failed && s->n_nodes >= 3) chain_cons_path(s, cp, s->scr[2], s->n_cap);
     if (threadIdx.x == 0) {
-        if (run_cons && !s->failed && s->n_nodes >= 3) chain_consensus(s, cp, s->scr[2], s->n_cap);
         const int msa_len = chain_msa_rank(s, cp);
         long long at = -1;
         if (msa_len > 0) {
@@ -201,7 +203,7 @@ __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_msa_kernel(PoaChainSlot
 }
 
 /* GFA of every finished group, one CTA per group: order and size on one thread (chain_gfa_size), the record by the
- * whole CTA (chain_gfa_record).  with_cons: the record carries the consensus path chain_consensus left in scr[1] --
+ * whole CTA (chain_gfa_record).  with_cons: the record carries the consensus path chain_cons_path left in scr[1] --
  * run_cons: compute that path here (the consensus kernel did not run).  Records share the consensus records' cursor at
  * word rec_base + cursor, each 8-byte aligned; rec_off[g] = -1 if the group has none (it is then finished by the launch
  * engine). */
@@ -212,8 +214,8 @@ __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_gfa_kernel(PoaChainSlot
     __shared__ long long at_s;
     __shared__ int32_t hdr_s[POA_GFA_HDR_WORDS];
     PoaChainSlot *s = &slots[blockIdx.x];
+    if (run_cons && !s->failed && s->n_nodes >= 3) chain_cons_path(s, cp, s->scr[2], s->n_cap);
     if (threadIdx.x == 0) {
-        if (run_cons && !s->failed && s->n_nodes >= 3) chain_consensus(s, cp, s->scr[2], s->n_cap);
         const long long words = chain_gfa_size(s, cp, with_cons, hdr_s);
         long long at = -1;
         if (words > 0) {
@@ -237,9 +239,12 @@ int poa_chain_eligible(const abpoa_para_t *abpt) {
     { const char *np = getenv("ABPOA_GPU_NO_P16"); if (np && *np == '1') return 0; }      /* the chain only has the packed int16 kernel */
     if (abpt->align_mode != ABPOA_GLOBAL_MODE || abpt->wb < 0) return 0;
     if (abpt->gap_mode == ABPOA_LINEAR_GAP) return 0;                      /* banded linear gaps: generic kernel only (lane-exact band edges) */
-    /* RC-MSA and GFA run on the chain (per-node read sets, poa_chain_msa_kernel / poa_chain_gfa_kernel); use_read_ids is
-     * what abpoa_post_set_para sets for them */
-    if ((abpt->use_read_ids && !abpt->out_msa && !abpt->out_gfa) || abpt->max_n_cons > 1 || abpt->cons_algrm != ABPOA_HB) return 0;
+    /* RC-MSA and GFA run on the chain (per-node read sets, poa_chain_msa_kernel / poa_chain_gfa_kernel), and so does the
+     * single-cluster most-frequent-base consensus (it needs n_read per node only; under sub_aln it needs n_span_read,
+     * which the device does not keep); use_read_ids is what abpoa_post_set_para sets for them */
+    const int mf = abpt->cons_algrm == ABPOA_MF && abpt->use_read_ids && !abpt->sub_aln;
+    if (abpt->cons_algrm != ABPOA_HB && !mf) return 0;
+    if ((abpt->use_read_ids && !abpt->out_msa && !abpt->out_gfa && !mf) || abpt->max_n_cons > 1) return 0;
     if (abpt->use_qv || abpt->amb_strand || abpt->inc_path_score || abpt->zdrop > 0 || abpt->rev_cigar || !abpt->ret_cigar) return 0;
     if (abpt->put_gap_on_right || abpt->put_gap_at_end) return 0;         /* handled by the kernels, but keep the chain on the common configuration */
     if (abpt->m > POA_MAX_M) return 0;
@@ -327,6 +332,7 @@ struct ChainCall {
     bool free_run;          /* free-running schedule (default); else lock-step rounds, two kernels per round and cohort */
     int cohorts;            /* round schedule: ABPOA_GPU_CHAIN_COHORTS, or 0: as many as keep each alignment grid to one CTA per SM */
     bool want_msa; int with_cons;
+    bool mf;                /* most-frequent-base consensus (-a 1); heaviest bundling otherwise */
     bool want_gfa;          /* GFA records: out_gfa with a writer attached (without one, the reference prints and computes nothing) */
     int W;                  /* RC-MSA / GFA: words per read set (W of the largest group), 0 otherwise */
     bool export_graph;      /* the whole graph comes back (compact export) and the host computes the consensus on it */
@@ -350,6 +356,7 @@ ChainCall chain_call(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_worker
     c.want_msa = abpt->out_msa && !abpt->out_gfa;           /* with out_gfa, abpoa_output prints only the GFA */
     c.want_gfa = abpt->out_gfa && emit != NULL;
     c.with_cons = abpt->out_cons ? 1 : 0;
+    c.mf = abpt->cons_algrm == ABPOA_MF;
     c.W = 0;
     if (c.want_msa || c.want_gfa) for (int g : todo) c.W = std::max(c.W, (groups[g].n_seq + 63) / 64);
     c.sm_count = 132;
@@ -593,6 +600,7 @@ struct Wave {
         PoaChainParams hcp; memset(&hcp, 0, sizeof hcp);
         hcp.K = c.K; hcp.A = c.A; hcp.m = c.m; hcp.max_mat = abpt->max_mat; hcp.min_mis = abpt->min_mis; hcp.o1 = abpt->gap_open1; hcp.e1 = abpt->gap_ext1;
         hcp.oe1 = abpt->gap_open1 + abpt->gap_ext1; hcp.oe2 = abpt->gap_open2 + abpt->gap_ext2; hcp.record = c.record ? 1 : 0; hcp.P = c.P; hcp.W = c.W;
+        hcp.cons_algrm = c.mf ? 1 : 0;
         PoaParamsDev hprm; poa_fill_params(&hprm, c.abpt, 15);
         CK(cudaMemcpyAsync(d_reads, h_reads, reads_bytes, cudaMemcpyHostToDevice, s0));
         CK(cudaMemcpyAsync(d_slots, hs.data(), (size_t)nw * sizeof(PoaChainSlot), cudaMemcpyHostToDevice, s0));
@@ -713,7 +721,7 @@ struct Wave {
     }
 
     /* Join the cohort streams, run the result kernels and copy back what the host needs; the arena borrow ends here.
-     * Default: heaviest-bundling consensus on the device, only consensus bytes come back.  export_graph: the whole graph
+     * Default: the consensus on the device (chain_cons_path), only consensus bytes come back.  export_graph: the whole graph
      * comes back (compact export) and the host layer computes the consensus on it -- the cross-check of the device graph
      * against the host code.  RC-MSA: the rows are always the device's (poa_chain_msa_kernel); -r1 needs no consensus.
      * GFA: the record is always the device's (poa_chain_gfa_kernel); -r3 needs no consensus, and without a writer neither
@@ -733,7 +741,7 @@ struct Wave {
         rec_base = export_graph ? (unsigned long long)ex_words : 0;
         if (export_graph) poa_chain_export_kernel<<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw, d_ex, d_exoff, d_excap);
         if (any_rec) CK(cudaMemsetAsync(d_ccur, 0, sizeof(unsigned long long), s0));
-        if (cons_kernel) poa_chain_consensus_kernel<<<nw, 32, 0, s0>>>(d_slots, d_cp, nw, d_ex, d_ccur, (unsigned long long)(pool_bytes / 4), d_recoff);
+        if (cons_kernel) poa_chain_consensus_kernel<<<nw, c.mf ? POA_CHAIN_T : 32, 0, s0>>>(d_slots, d_cp, nw, d_ex, d_ccur, (unsigned long long)(pool_bytes / 4), d_recoff);
         CK(cudaGetLastError());
         launches += (export_graph || cons_kernel) ? 1 : 0;
         if (want_msa) {

@@ -65,6 +65,7 @@ typedef struct PoaChainParams {         /* one per batch call */
     int32_t P;                          /* plane units per 8-cell group of a DP row (compact layout:
                                            H and the E planes; 1 / 2 / 3) */
     int32_t W;                          /* 64-bit words per read set (ceil(n_reads / 64) of the largest group); 0: no RC-MSA */
+    int32_t cons_algrm;                 /* consensus: 0 heaviest bundling (ABPOA_HB), 1 most frequent base (ABPOA_MF) */
 } PoaChainParams;
 
 typedef struct PoaChainSlot {           /* one per read group; every pointer aims into the group's HBM region */
@@ -633,7 +634,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
 }
 
 /* ------------------------------------------------------------------ consensus on the device (SURVEY 8f row f2)
- * Heaviest bundling, single cluster (reference src/abpoa_output.c:477-547; host twin: heaviest_bundling in
+ * Heaviest bundling (most frequent base: chain_mf_consensus below), single cluster (reference src/abpoa_output.c:477-547; host twin: heaviest_bundling in
  * poa_cons.c): score[v] = w(best out-edge) + score[its head], best = largest weight, among equal weights an inner
  * node keeps the LAST edge whose head scores >= the current pick, SRC keeps the first unless strictly better.
  * The reference visits nodes in reverse Kahn order; the values depend only on the out-neighbours, so one backward
@@ -717,6 +718,67 @@ POA_DEV int chain_msa_rank(PoaChainSlot *s, const PoaChainParams *cp) {
         }
     }
     return -1;
+}
+
+/* Most frequent base per RC-MSA column, single cluster (reference src/abpoa_output.c:393-451, :549-586; host twin:
+ * most_frequent in poa_cons.c).  Ranks on one thread (chain_msa_rank: scr[3..5]), the vote and the compaction by the
+ * whole CTA.  An aligned set takes one rank when it is pushed and popped, and every column is exactly one aligned set:
+ * its members' bases are pairwise distinct (a read reuses a sibling with its base before it adds a node), so the
+ * reference's per-column table, where a later node overwrites an earlier one of the same base, never overwrites.  The
+ * set's smallest id votes it: codes 0..m-2 only, the largest n_read wins, the lowest code among equal counts; the column
+ * is kept iff that count >= n_reads minus the votes.  Writes the record of chain_consensus (out[0] = length, then
+ * base | coverage << 8) and leaves the path as nxt[] in scr[1] (nxt[0] = first node, the last points to SINK) for
+ * chain_msa_rows and chain_gfa_record; scr[0] holds the kept ids.  Needs the whole CTA. */
+POA_DEV void chain_mf_consensus(PoaChainSlot *s, const PoaChainParams *cp, int32_t *out, int out_cap) {
+    POA_SHARED int msa_len_s;
+    if (POA_TID0) msa_len_s = chain_msa_rank(s, cp);
+    POA_CTA_SYNC();
+    const int msa_len = msa_len_s;
+    if (msa_len < 0) { if (POA_TID0) out[0] = -1; POA_CTA_SYNC(); return; }
+    const int A = cp->A, m = cp->m, n = s->n_nodes, n_seq = s->n_reads;
+    const int32_t *rank = s->scr[5];
+    int32_t *win = s->scr[3], *pos = s->scr[4], *kept = s->scr[0], *nxt = s->scr[1];       /* the rank pass's deg / stack are dead */
+    POA_PAR_FOR(j, msa_len) win[j] = -1;
+    POA_CTA_SYNC();
+    POA_PAR_FOR(v, n) {
+        const int na = s->aln_cnt[v];
+        const int32_t *al = s->aln_id + (size_t)v * A;
+        int lead = v >= 2, r = rank[v];
+        for (int a = 0; a < na; ++a) { if (al[a] < v) lead = 0; if (rank[al[a]] > r) r = rank[al[a]]; }
+        if (lead) {
+            int max_c = 0, max_b = m, total_c = 0, pick = -1;
+            for (int a = -1; a < na; ++a) {
+                const int u = a < 0 ? v : al[a], b = s->base[u];
+                if (b >= m - 1) continue;
+                const int c = s->n_read[u];
+                total_c += c;
+                if (c > max_c || (c == max_c && c > 0 && b < max_b)) { max_c = c; max_b = b; pick = u; }
+            }
+            if (pick >= 0 && max_c >= n_seq - total_c) win[r - 1] = pick;
+        }
+    }
+    POA_CTA_SYNC();
+    POA_PAR_FOR(j, msa_len) pos[j] = win[j] >= 0;
+    POA_CTA_SYNC();
+    const int len = cta_excl_scan(pos, msa_len);
+    POA_CTA_SYNC();
+    if (1 + len > out_cap) { if (POA_TID0) out[0] = -1; POA_CTA_SYNC(); return; }
+    POA_PAR_FOR(j, msa_len) {
+        const int v = win[j];
+        if (v >= 0) { out[1 + pos[j]] = (int32_t)s->base[v] | (s->n_read[v] << 8); kept[pos[j]] = v; }
+    }
+    POA_CTA_SYNC();
+    POA_PAR_FOR(k, len) nxt[kept[k]] = k + 1 < len ? kept[k + 1] : 1;
+    if (POA_TID0) { out[0] = len; nxt[0] = len > 0 ? kept[0] : 1; }
+    POA_CTA_SYNC();
+}
+
+/* The consensus the call asked for (PoaChainParams::cons_algrm): the record in `out`, the path in scr[1].  Heaviest
+ * bundling runs on thread 0 (the other threads return at once), most frequent base on the whole CTA: every thread of
+ * the CTA calls this. */
+POA_DEV void chain_cons_path(PoaChainSlot *s, const PoaChainParams *cp, int32_t *out, int out_cap) {
+    if (cp->cons_algrm == 1) chain_mf_consensus(s, cp, out, out_cap);
+    else chain_consensus(s, cp, out, out_cap);
 }
 
 /* Rows of the RC-MSA (host twin: abpoa_generate_rc_msa in poa_cons.c) from the ranks of chain_msa_rank: n_reads rows (+ the

@@ -4,13 +4,14 @@
  * that parity with the reference can be expressed on its own outputs (consensus FASTA,
  * RC-MSA).  Behaviour follows
  *   heaviest bundling   reference src/abpoa_output.c:477-547 (tie rules!), :375-391
+ *   most frequent base  reference src/abpoa_output.c:393-451, :549-586 (-a 1)
  *   phred of a column   reference src/abpoa_output.c:296-302
  *   RC-MSA              reference src/abpoa_output.c:105-192
  *   writers             reference src/abpoa_output.c:72-103, :588-627
  *   GFA                 reference src/abpoa_output.c:194-294
  *   abpoa_output        reference src/abpoa_align.c:354-370
  * Out of the hot-path scope and therefore not provided (they abort with a message):
- * most-frequent-base consensus, multi-consensus clustering (max_n_cons > 1), dot.
+ * multi-consensus clustering (max_n_cons > 1), consensus algorithms other than -a 0 / -a 1, dot.
  */
 #include <math.h>
 #include "poa_internal.h"
@@ -104,14 +105,59 @@ static void heaviest_bundling(abpoa_graph_t *abg, abpoa_cons_t *abc) {
     free(deg); free(score); free(next); free(q);
 }
 
+static int msa_column(const abpoa_graph_t *abg, int id);
+
+/* Most frequent base per RC-MSA column, single cluster (device twin: chain_mf_consensus in poa_chain.cuh).  Every node
+ * (ascending id) sets weight n_read and node id for its base in its column, a later node overwriting an earlier one.  A
+ * column votes with codes 0..m-2 only (code m-1, N or the last amino-acid code, counts as gap): the strictly largest
+ * count wins, so the lowest code among equal counts; the column is kept iff that count >= the gap count, n_seq minus
+ * the votes (under sub_aln the winner's n_span_read minus the votes). */
+static void most_frequent(abpoa_graph_t *abg, const abpoa_para_t *abpt, abpoa_cons_t *abc) {
+    const int m = abpt->m, n_seq = abc->n_seq;
+    poa_set_msa_rank(abg, ABPOA_SRC_NODE_ID, ABPOA_SINK_NODE_ID);
+    const int msa_len = abg->node_id_to_msa_rank[ABPOA_SINK_NODE_ID] - 1;
+    int *w = (int *)poa_xcalloc((size_t)POA_MAX(msa_len, 1) * m, sizeof(int));
+    int *id = (int *)poa_xcalloc((size_t)POA_MAX(msa_len, 1) * m, sizeof(int));
+    abc->clu_n_seq[0] = n_seq;
+    for (int i = 0; i < n_seq; ++i) abc->clu_read_ids[0][i] = i;
+    for (int i = 2; i < abg->node_n; ++i) {
+        const int col = msa_column(abg, i) - 1, b = abg->node[i].base;
+        w[(size_t)col * m + b] = abg->node[i].n_read;
+        id[(size_t)col * m + b] = i;
+    }
+    int len = 0;
+    for (int col = 0; col < msa_len; ++col) {
+        const int *cw = w + (size_t)col * m;
+        int max_c = 0, max_base = m, total_c = 0;
+        for (int b = 0; b < m - 1; ++b) {
+            if (cw[b] > max_c) { max_c = cw[b]; max_base = b; }
+            total_c += cw[b];
+        }
+        /* no vote: never kept without sub_aln (gap = n_seq); under sub_aln the reference reads past the column's row */
+        if (max_base == m) continue;
+        const int node_id = id[(size_t)col * m + max_base];
+        const int gap_c = (abpt->sub_aln ? abg->node[node_id].n_span_read : n_seq) - total_c;
+        if (max_c < gap_c) continue;
+        abc->cons_node_ids[0][len] = node_id;
+        abc->cons_base[0][len] = (uint8_t)max_base;
+        abc->cons_cov[0][len] = max_c;
+        abc->cons_phred_score[0][len] = column_phred(max_c, n_seq);
+        ++len;
+    }
+    abc->cons_len[0] = len;
+    free(w); free(id);
+}
+
 void abpoa_generate_consensus(abpoa_t *ab, abpoa_para_t *abpt) {
     abpoa_graph_t *abg = ab->abg;
     poa_graph_sync_public(abg);
     if (abg->is_called_cons == 1 || abg->node_n <= 2) return;
     if (abpt->max_n_cons > 1) poa_die(__func__, "multi-consensus clustering (max_n_cons > 1) is outside the scope of the GPU hot-path library.");
-    if (abpt->cons_algrm != ABPOA_HB) poa_die(__func__, "most-frequent-base consensus is outside the scope of the GPU hot-path library.");
+    if (abpt->cons_algrm != ABPOA_HB && abpt->cons_algrm != ABPOA_MF)
+        poa_die(__func__, "unknown consensus algorithm %d (0: heaviest bundling, 1: most frequent base).", abpt->cons_algrm);
     cons_alloc(ab->abc, abg->node_n, ab->abs->n_seq, 1);
-    heaviest_bundling(abg, ab->abc);
+    if (abpt->cons_algrm == ABPOA_HB) heaviest_bundling(abg, ab->abc);
+    else most_frequent(abg, abpt, ab->abc);
     abg->is_called_cons = 1;
 }
 
