@@ -28,7 +28,8 @@
  *
  * Scope of the chain: global alignment, banded (wb >= 0), packed-int16 admissible scores, heaviest-bundling or
  * most-frequent-base consensus (single cluster, no sub_aln), row-column MSA and GFA (one read set per node, not per
- * edge), unit base weights.  Everything else takes the other engine.
+ * edge), unit base weights, ambiguous strand (-s: the alignment warp retries a weak hit as the reverse complement,
+ * chain_align_read in poa_kernels.cu).  Everything else takes the other engine.
  */
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -53,9 +54,9 @@
     poa_die("libabpoa_b200/chain", "%s failed at %s:%d: %s", #call, __FILE__, __LINE__, cudaGetErrorString(e_)); } while (0)
 
 extern "C" cudaError_t poa_launch_chain_dp_worker(int gap_mode, const int *gaps, PoaChainSlot *slots, PoaChainSync *sync, int n_groups,
-                                                  const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st);
+                                                  const PoaChainParams *cp, int strand, const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st);
 extern "C" cudaError_t poa_launch_chain_align_p16(int gap_mode, const int *gaps, const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round,
-                                                  const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st);
+                                                  const PoaChainParams *cp, int strand, const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st);
 extern "C" void poa_pick_ring(int gap_mode, int bits, int band_cells, size_t smem_budget, int *ring_rows, int *ring_cells);
 
 static_assert(offsetof(PoaChainSync, q_tail) == 128 && offsetof(PoaChainSync, total) == 256 && offsetof(PoaChainSync, abort) == 384,
@@ -245,7 +246,7 @@ int poa_chain_eligible(const abpoa_para_t *abpt) {
     const int mf = abpt->cons_algrm == ABPOA_MF && abpt->use_read_ids && !abpt->sub_aln;
     if (abpt->cons_algrm != ABPOA_HB && !mf) return 0;
     if ((abpt->use_read_ids && !abpt->out_msa && !abpt->out_gfa && !mf) || abpt->max_n_cons > 1) return 0;
-    if (abpt->use_qv || abpt->amb_strand || abpt->inc_path_score || abpt->zdrop > 0 || abpt->rev_cigar || !abpt->ret_cigar) return 0;
+    if (abpt->use_qv || abpt->inc_path_score || abpt->zdrop > 0 || abpt->rev_cigar || !abpt->ret_cigar) return 0;
     if (abpt->put_gap_on_right || abpt->put_gap_at_end) return 0;         /* handled by the kernels, but keep the chain on the common configuration */
     if (abpt->m > POA_MAX_M) return 0;
     if (!(abpt->disable_seeding && abpt->progressive_poa == 0)) return 0;
@@ -257,6 +258,10 @@ namespace {
 /* the round schedule keeps every group listed this many rounds beyond its last read: a group that has to re-run an
  * alignment (band wider than its plane slab) falls one round behind (slots with nothing to do return at once) */
 const int ROUNDS_EXTRA = 2;
+/* ... and with -s one more round per read: the forward pass of a read that arrives reverse-complemented wanders off the
+ * band estimate often, and every read may be re-run once */
+int rounds_extra(bool strand, int n_reads) { return ROUNDS_EXTRA + (strand ? n_reads - 1 : 0); }
+const double STRAND_SLAB_X = 5.0;       /* -s: plane estimate factor (plan_groups) */
 
 struct GroupPlan {
     int g;                  /* index into the caller's groups */
@@ -336,6 +341,7 @@ struct ChainCall {
     bool want_gfa;          /* GFA records: out_gfa with a writer attached (without one, the reference prints and computes nothing) */
     int W;                  /* RC-MSA / GFA: words per read set (W of the largest group), 0 otherwise */
     bool export_graph;      /* the whole graph comes back (compact export) and the host computes the consensus on it */
+    bool strand;            /* -s: the alignment warp retries weak hits as the reverse complement; read_rc comes back */
     int sm_count;
 };
 
@@ -357,6 +363,7 @@ ChainCall chain_call(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_worker
     c.want_gfa = abpt->out_gfa && emit != NULL;
     c.with_cons = abpt->out_cons ? 1 : 0;
     c.mf = abpt->cons_algrm == ABPOA_MF;
+    c.strand = abpt->amb_strand != 0;
     c.W = 0;
     if (c.want_msa || c.want_gfa) for (int g : todo) c.W = std::max(c.W, (groups[g].n_seq + 63) / 64);
     c.sm_count = 132;
@@ -387,7 +394,7 @@ std::vector<GroupPlan> plan_groups(const ChainCall &c, const std::vector<int> &t
         /* what the wave carve will take for the group, at its 256-byte granularity */
         PoaChainSlot probe;
         size_t own = 0; p.reads_bytes = 0;
-        chain_slot_layout(&probe, p.n_cap, p.qmax, p.n_reads, c.K, c.A, c.m, c.W, c.record, [&](size_t b) { own += al256(b); return (uint8_t *)NULL; });
+        chain_slot_layout(&probe, p.n_cap, p.qmax, p.n_reads, c.K, c.A, c.m, c.W, c.record, [&](size_t b) { own += al256(b); return (uint8_t *)NULL; }, c.strand);
         chain_slot_reads(&probe, p.n_reads, p.bases, [&](size_t b) { p.reads_bytes += al256(b); return (uint8_t *)NULL; });
         p.static_bytes = own + p.reads_bytes;
         const size_t nc = (size_t)p.n_cap;
@@ -407,6 +414,10 @@ std::vector<GroupPlan> plan_groups(const ChainCall &c, const std::vector<int> &t
         const int band_slack = c.free_run ? 0 : 32;
         const double rows_final = std::min<double>(2.0 + (double)p.bases, (double)p.qmax * (1.0 + growth * (p.n_reads - 1)) + 64);
         p.pool_units_est = rows_final * (double)((2 * wmax + 1 + band_slack + 7) / 8 + 2) * c.P;
+        /* -s: a read that arrives reverse-complemented is first aligned on the wrong strand, and that alignment's band
+         * wanders far off the estimate (50 x 10 kbp convex, every third read flipped: slabs of 1.5x the estimate handed
+         * 706 of 1000 groups back, slabs of about 6x none).  Fewer groups per wave, each with a larger slab. */
+        if (c.strand) p.pool_units_est *= STRAND_SLAB_X;
         plans.push_back(p);
     }
     return plans;
@@ -467,7 +478,7 @@ struct Wave {
     std::vector<PoaChainSlot> hs, fin;      /* the slots as uploaded / as they came back */
     uint8_t *h_reads = NULL; int32_t *h_cons = NULL, *h_ex = NULL;
     std::vector<int64_t> h_exoff; std::vector<int32_t> h_excap; int64_t ex_words = 0;
-    int max_reads = 0, band_cells = 64;
+    int band_cells = 64;
     /* streams and events */
     std::vector<Cohort> coh;
     cudaStream_t s0 = NULL, st_dp = NULL;
@@ -477,6 +488,7 @@ struct Wave {
     bool cons_kernel = false; unsigned long long rec_base = 0, cons_words = 0;
     std::vector<int64_t> recoff, msaoff, gfaoff, words, hoff2; int64_t tot_words = 0;
     std::vector<std::vector<int32_t>> rs, rn; std::vector<std::vector<uint64_t>> rh;
+    std::vector<std::vector<uint8_t>> rc;  /* -s: read_rc of every group */
     int n_failed = 0;
     /* accounting */
     int64_t launches = 0; uint64_t h2d = 0, d2h = 0; float dev_ms = 0.f;
@@ -537,7 +549,7 @@ struct Wave {
             const GroupPlan &p = plans[t];
             const abpoa_gpu_group_t &in = c.groups[p.g];
             PoaChainSlot &s = hs[t]; memset(&s, 0, sizeof s);
-            chain_slot_layout(&s, p.n_cap, p.qmax, p.n_reads, c.K, c.A, c.m, c.W, c.record, gtake);
+            chain_slot_layout(&s, p.n_cap, p.qmax, p.n_reads, c.K, c.A, c.m, c.W, c.record, gtake, c.strand);
             chain_slot_reads(&s, p.n_reads, p.bases, rtake);
             int32_t *hoff = (int32_t *)(h_reads + ((const uint8_t *)s.read_off - d_reads)), *hw = (int32_t *)(h_reads + ((const uint8_t *)s.read_w - d_reads));
             int acc = 0;
@@ -548,7 +560,6 @@ struct Wave {
                 if (bc > band_cells) band_cells = bc;
             }
             hoff[p.n_reads] = acc;
-            if (p.n_reads > max_reads) max_reads = p.n_reads;
         }
         /* the read bytes themselves: half a gigabyte at BASELINE size, copied into the pinned buffer by all workers */
         {
@@ -567,9 +578,10 @@ struct Wave {
             for (auto &x : th) x.join();
         }
         t_staged = now_ms();
-        /* round index lists (run_rounds): every group is listed from round 1 to ROUNDS_EXTRA rounds past its last read.
+        /* round index lists (run_rounds): every group is listed from round 1 to rounds_extra() rounds past its last read.
          * Reserved on both schedules: the wave's layout up to the plane pool does not depend on the schedule. */
-        idx_n = (size_t)n_tasks + (size_t)ROUNDS_EXTRA * nw;
+        idx_n = (size_t)n_tasks;
+        for (int t = 0; t < nw; ++t) idx_n += (size_t)rounds_extra(c.strand, plans[t].n_reads);
         d_idx = (int32_t *)dtake(std::max<size_t>(idx_n, 1) * 4);
         /* export buffers */
         h_exoff.resize((size_t)nw); h_excap.resize((size_t)nw);
@@ -600,7 +612,7 @@ struct Wave {
         PoaChainParams hcp; memset(&hcp, 0, sizeof hcp);
         hcp.K = c.K; hcp.A = c.A; hcp.m = c.m; hcp.max_mat = abpt->max_mat; hcp.min_mis = abpt->min_mis; hcp.o1 = abpt->gap_open1; hcp.e1 = abpt->gap_ext1;
         hcp.oe1 = abpt->gap_open1 + abpt->gap_ext1; hcp.oe2 = abpt->gap_open2 + abpt->gap_ext2; hcp.record = c.record ? 1 : 0; hcp.P = c.P; hcp.W = c.W;
-        hcp.cons_algrm = c.mf ? 1 : 0;
+        hcp.cons_algrm = c.mf ? 1 : 0; hcp.amb_strand = c.strand ? 1 : 0;
         PoaParamsDev hprm; poa_fill_params(&hprm, c.abpt, 15);
         CK(cudaMemcpyAsync(d_reads, h_reads, reads_bytes, cudaMemcpyHostToDevice, s0));
         CK(cudaMemcpyAsync(d_slots, hs.data(), (size_t)nw * sizeof(PoaChainSlot), cudaMemcpyHostToDevice, s0));
@@ -662,10 +674,10 @@ struct Wave {
         CK(cudaFuncSetAttribute(poa_chain_fuse_worker_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
         static const bool dp_first = [] { const char *e = getenv("ABPOA_GPU_CHAIN_DP_FIRST"); return e && *e == '1'; }();     /* experiment */
         CK(cudaStreamWaitEvent(st_dp, ev_sync, 0));
-        if (dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_prm, ring_rows, ring_cells, st_dp));
+        if (dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, d_prm, ring_rows, ring_cells, st_dp));
         poa_chain_fuse_worker_kernel<<<n_fuse, POA_CHAIN_T, 0, s0>>>(d_slots, d_sync, d_cp);
         CK(cudaGetLastError());
-        if (!dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_prm, ring_rows, ring_cells, st_dp));
+        if (!dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, d_prm, ring_rows, ring_cells, st_dp));
         cudaEvent_t ev_dp; CK(cudaEventCreateWithFlags(&ev_dp, cudaEventDisableTiming));
         CK(cudaEventRecord(ev_dp, st_dp));
         CK(cudaStreamWaitEvent(s0, ev_dp, 0));
@@ -693,11 +705,12 @@ struct Wave {
         }
         /* round index lists per cohort: wave-local slot indices of the groups that still have a read r */
         std::vector<int32_t> h_idx; std::vector<std::vector<std::pair<size_t, int>>> round_of(coh.size());   /* (offset into h_idx, count) per round */
-        const int n_rounds = max_reads - 1 + ROUNDS_EXTRA;
+        int n_rounds = 0;
+        for (int t = 0; t < nw; ++t) n_rounds = std::max(n_rounds, plans[t].n_reads - 1 + rounds_extra(c.strand, plans[t].n_reads));
         for (size_t k = 0; k < coh.size(); ++k)
             for (int r = 1; r <= n_rounds; ++r) {
                 const size_t at = h_idx.size(); int cnt = 0;
-                for (int t : coh[k].members) if (plans[t].n_reads + ROUNDS_EXTRA > r) { h_idx.push_back(t); ++cnt; }
+                for (int t : coh[k].members) if (plans[t].n_reads + rounds_extra(c.strand, plans[t].n_reads) > r) { h_idx.push_back(t); ++cnt; }
                 round_of[k].push_back({at, cnt});
             }
         if (h_idx.size() != idx_n) poa_die("libabpoa_b200/chain", "round index lists (%zu entries) do not fill their region (%zu)", h_idx.size(), idx_n);
@@ -711,7 +724,7 @@ struct Wave {
                 cudaEvent_t e0, e1, e2; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1)); CK(cudaEventCreate(&e2));
                 coh[k].marks.push_back(e0); coh[k].marks.push_back(e1); coh[k].marks.push_back(e2);
                 CK(cudaEventRecord(e0, st));
-                CK(poa_launch_chain_align_p16(c.abpt->gap_mode, gaps, d_slots, d_idx + ro.first, ro.second, r, d_prm, ring_rows, ring_cells, st));
+                CK(poa_launch_chain_align_p16(c.abpt->gap_mode, gaps, d_slots, d_idx + ro.first, ro.second, r, d_cp, c.strand, d_prm, ring_rows, ring_cells, st));
                 CK(cudaEventRecord(e1, st));
                 poa_chain_fuse_kernel<<<ro.second, POA_CHAIN_T, 0, st>>>(d_slots, d_idx + ro.first, d_cp, ro.second, r);
                 CK(cudaGetLastError());
@@ -815,8 +828,16 @@ struct Wave {
             CK(cudaMemcpyAsync(rn[t].data(), fin[t].rec_nops, (size_t)nr * 4, cudaMemcpyDeviceToHost, s0));
             CK(cudaMemcpyAsync(rh[t].data(), fin[t].rec_hash, (size_t)nr * 8, cudaMemcpyDeviceToHost, s0));
         }
+        /* -s: which reads were fused as their reverse complement */
+        rc.resize((size_t)nw);
+        uint64_t rc_bytes = 0;
+        if (c.strand) for (int t = 0; t < nw; ++t) {
+            rc[t].resize((size_t)plans[t].n_reads);
+            CK(cudaMemcpyAsync(rc[t].data(), fin[t].read_rc, (size_t)plans[t].n_reads, cudaMemcpyDeviceToHost, s0));
+            rc_bytes += (uint64_t)plans[t].n_reads;
+        }
         CK(cudaStreamSynchronize(s0));
-        d2h = (uint64_t)tot_words * 4 + (uint64_t)cons_words * 4 + (uint64_t)nw * (sizeof(PoaChainSlot) + 16);
+        d2h = (uint64_t)tot_words * 4 + (uint64_t)cons_words * 4 + (uint64_t)nw * (sizeof(PoaChainSlot) + 16) + rc_bytes;
         poa_arena_return(c.arena, d_base, total); d_base = NULL;
         t_copied = now_ms();
     }
@@ -845,7 +866,11 @@ struct Wave {
                     abpoa_reset(ab, abpt, p.qmax);
                     abpoa_seq_t *abs = ab->abs;
                     abs->n_seq = p.n_reads; poa_seq_reserve(abs);
-                    for (int i = 0; i < p.n_reads; ++i) { abs->is_rc[i] = 0; abs->name[i].l = 0; }
+                    int n_rc_dp = 0;                           /* -s: second alignments (the reverse complement of a weak hit) */
+                    for (int i = 0; i < p.n_reads; ++i) {
+                        abs->is_rc[i] = c.strand ? rc[t][i] & 1 : 0; abs->name[i].l = 0;
+                        if (c.strand) n_rc_dp += rc[t][i] >> 1 & 1;
+                    }
                     if (c.export_graph) poa_graph_import(ab, abpt, h_ex + hoff2[t]);
                     else if (cons_kernel) {                    /* the device's consensus: base | coverage << 8 per position */
                         const int32_t *rec = h_cons + recoff[t];
@@ -861,7 +886,7 @@ struct Wave {
                     if (c.want_gfa) poa_gfa_install(ab, h_cons + (gfaoff[t] - (int64_t)rec_base));     /* printed by abpoa_generate_gfa */
                     poa_finish_group_result(ab, abpt, o, c.emit, p.g);
                     if (c.want_gfa) poa_gfa_install(ab, NULL);
-                    o->dp_cells = fin[t].cells; o->n_aligned = p.n_reads - 1;
+                    o->dp_cells = fin[t].cells; o->n_aligned = p.n_reads - 1 + n_rc_dp;     /* the launch engine counts every DP */
                     if (c.record) {
                         const int nr = p.n_reads;
                         o->read_best_score = (int32_t *)poa_xcalloc((size_t)nr, sizeof(int32_t));

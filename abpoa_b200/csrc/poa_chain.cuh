@@ -66,6 +66,7 @@ typedef struct PoaChainParams {         /* one per batch call */
                                            H and the E planes; 1 / 2 / 3) */
     int32_t W;                          /* 64-bit words per read set (ceil(n_reads / 64) of the largest group); 0: no RC-MSA */
     int32_t cons_algrm;                 /* consensus: 0 heaviest bundling (ABPOA_HB), 1 most frequent base (ABPOA_MF) */
+    int32_t amb_strand;                 /* -s: a weak forward hit is re-aligned as the reverse complement (chain_weak_hit) */
 } PoaChainParams;
 
 typedef struct PoaChainSlot {           /* one per read group; every pointer aims into the group's HBM region */
@@ -106,14 +107,21 @@ typedef struct PoaChainSlot {           /* one per read group; every pointer aim
     /* RC-MSA (PoaChainParams::W > 0): bit r of node v's set = read r's path passes through v, i.e. the union of the read
      * sets of v's out-edges in the host graph -- all the row-column MSA needs (reference src/abpoa_output.c:105-192) */
     uint64_t *read_set;                                 /* [n_cap * W] */
+    /* -s (PoaChainParams::amb_strand): per read, bit 0 = fused as the reverse complement, bit 1 = the reverse complement was
+     * aligned too (a weak forward hit); the alignment warp runs that second pass into rc_cigar / rc_result */
+    uint8_t *read_rc;                                   /* [n_reads] */
+    uint64_t *rc_cigar;                                 /* [jd.cigar_cap] */
+    PoaResultDev *rc_result;
 } PoaChainSlot;
 
 /* A group's memory, host side: the slot's capacities and every per-group array, taken in one fixed order from the
  * caller's allocator `take(bytes)`, which also decides the alignment.  The engine carves a wave's HBM with it, its
  * wave planner sums the same requests, and the CPU emulator lays out its host buffer with it, so the three cannot
- * disagree.  The reads (chain_slot_reads) live in a region of their own: they are staged and uploaded in one copy. */
+ * disagree.  The reads (chain_slot_reads) live in a region of their own: they are staged and uploaded in one copy.
+ * `strand` (-s runs) adds the strand bytes and the second CIGAR buffer and result behind everything else. */
 template <class Take>
-static inline void chain_slot_layout(PoaChainSlot *s, int n_cap, int qmax, int n_reads, int K, int A, int m, int W, bool record, Take take) {
+static inline void chain_slot_layout(PoaChainSlot *s, int n_cap, int qmax, int n_reads, int K, int A, int m, int W, bool record, Take take,
+                                     bool strand = false) {
     const size_t nc = (size_t)n_cap, scr_n = nc > (size_t)qmax + 2 ? nc : (size_t)qmax + 2;
     s->n_cap = n_cap; s->pred_cap = (int32_t)(nc * 3); s->n_reads = n_reads;
     s->blob_cap = (int32_t)(256 + (nc + 1) * 8 + (size_t)s->pred_cap * 4 + 4 + (size_t)qmax + 64);
@@ -132,6 +140,11 @@ static inline void chain_slot_layout(PoaChainSlot *s, int n_cap, int qmax, int n
     s->jd.btrec = (PoaBtRec *)take(nc * sizeof(PoaBtRec));
     if (record) { s->rec_score = (int32_t *)take((size_t)n_reads * 4); s->rec_nops = (int32_t *)take((size_t)n_reads * 4); s->rec_hash = (uint64_t *)take((size_t)n_reads * 8); }
     if (W > 0) s->read_set = (uint64_t *)take(nc * W * 8);
+    if (strand) {
+        s->read_rc = (uint8_t *)take((size_t)n_reads);
+        s->rc_cigar = (uint64_t *)take((size_t)s->jd.cigar_cap * 8);
+        s->rc_result = (PoaResultDev *)take(sizeof(PoaResultDev));
+    }
 }
 
 /* the group's reads: `bases` bytes back to back, n_reads + 1 offsets, n_reads band half widths */
@@ -262,6 +275,23 @@ POA_DEV int chain_ref_pn(const PoaChainParams *cp, int qlen, int n_rows) {
 }
 
 POA_DEV size_t chain_al16(size_t x) { return (x + 15) & ~(size_t)15; }
+
+/* -s, reference src/abpoa_align.c:323-325: the forward hit is weak, so the reverse complement is aligned too.  node_n counts
+ * SRC and SINK (the job's n_rows); the bound is an int product times a double, as the reference evaluates it. */
+POA_DEV bool chain_weak_hit(int best_score, int qlen, int node_n, int max_mat) {
+    const int lim = qlen < node_n - 2 ? qlen : node_n - 2;
+    return best_score < lim * max_mat * .3333;
+}
+
+/* complement of a base code (reference src/abpoa_align.c:329): 0..3 -> 3..0, everything else -> 4, with -c too */
+POA_DEV uint8_t chain_comp(uint8_t b) { return b < 4 ? (uint8_t)(3 - b) : (uint8_t)4; }
+
+/* base qi of read r on the strand it is fused on: the reverse complement, computed on the fly, when read_rc[r] says so */
+POA_DEV uint8_t chain_read_base(const PoaChainSlot *s, int r, int qi) {
+    const uint8_t *q = s->reads + s->read_off[r];
+    if (s->read_rc && (s->read_rc[r] & 1)) return chain_comp(q[s->read_off[r + 1] - s->read_off[r] - 1 - qi]);
+    return q[qi];
+}
 
 /* ------------------------------------------------------------------ order-dependent passes */
 /* max_remain by row: remain[row] = remain[row of heaviest out-neighbour] + 1, SINK = -1 (reference
@@ -405,7 +435,7 @@ POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
         const int W = cp->W;
         POA_PAR_FOR(v, n) { uint64_t *rs = s->read_set + (size_t)v * W; for (int wd = 0; wd < W; ++wd) rs[wd] = (wd == 0 && v != 1) ? 1ull : 0ull; }
     }
-    if (POA_TID0) { s->n_nodes = n; s->cur = 0; s->fused = 1; s->retry = 0; }
+    if (POA_TID0) { s->n_nodes = n; s->cur = 0; s->fused = 1; s->retry = 0; if (s->read_rc) s->read_rc[0] = 0; }   /* read 0 seeds: no strand test */
     POA_CTA_SYNC();
     chain_set_remain(s, K, order, n);
     if (s->n_reads > 1) chain_flatten(s, cp, order, n, 1, /*pool_parity=*/1, 0);
@@ -438,7 +468,6 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
         return;
     }
     const int qlen = s->read_off[r + 1] - s->read_off[r];
-    const uint8_t *seq = s->reads + s->read_off[r];
     const uint64_t *ops = s->jd.cigar;
     const int n_ops = res->n_ops;
     const int old_n = s->n_nodes;
@@ -489,7 +518,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
         if (row == -2) POA_ATOMIC_OR(&s->failed, POA_CF_CIGAR);          /* global mode: every base is M or I */
         if (row >= 0) {
             const int v = order[row];
-            const uint8_t b = seq[qi];
+            const uint8_t b = chain_read_base(s, r, qi);
             if (s->base[v] == b) { kind = CK_OLD; target = v; }
             else {
                 const int na = s->aln_cnt[v]; const int32_t *al = s->aln_id + (size_t)v * A;
@@ -546,7 +575,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
         if (isnew[qi]) {
             const int id = old_n + newidx[qi];
             const int col = tgt[qi];                         /* CK_NEWM: the column's node */
-            s->base[id] = seq[qi]; s->in_cnt[id] = 0; s->out_cnt[id] = 0; s->aln_cnt[id] = 0; s->n_read[id] = 0;
+            s->base[id] = chain_read_base(s, r, qi); s->in_cnt[id] = 0; s->out_cnt[id] = 0; s->aln_cnt[id] = 0; s->n_read[id] = 0;
             if (cp->W > 0) for (int wd = 0; wd < cp->W; ++wd) s->read_set[(size_t)id * cp->W + wd] = 0;
             new_anchor[newidx[qi]] = kind_anchor[qi] & 0x0fffffff;      /* compacted: by new-node rank (anchors are non-decreasing) */
             item_row[qi] = col;                              /* remember the column for the aligned-set update */

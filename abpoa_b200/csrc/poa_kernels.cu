@@ -1794,14 +1794,62 @@ __global__ void POA_P16_BOUNDS poa_align_kernel_p16(const PoaJobDesc *__restrict
 
 static inline size_t ring_smem_bytes(int gap, int bits, int ring_rows, int ring_cells, int all_planes = 0);
 
+/* ------------------------------------------------------------------ one read of a chain group
+ * The job the fuse left in the slot (read sl->fused), on one warp.  STRAND (-s, PoaChainParams::amb_strand; the host
+ * picks the instantiation, so a run without -s compiles to the bare job): a weak forward hit (chain_weak_hit) is aligned
+ * again as the reverse complement, the reference's strand retry (src/abpoa_align.c:322-344).  The second pass writes the
+ * complemented bases over the blob's query and runs into rc_cigar / rc_result; it may overwrite qs, qprof, rowinfo, rowoff
+ * and btrec, which only the next flatten reads, and it rewrites them.  The reverse complement wins only if it scores
+ * strictly more; its CIGAR words and result are then copied over the primary ones, so the fuse reads one place either
+ * way.  The primary result carries the DP cells and cycles of both passes and the first status that is not OK (a failed
+ * pair is re-run or handed back like a failed alignment); read_rc[r] records the strand (bit 0) and whether the retry
+ * ran (bit 1). */
+template <int GAP, bool STRAND>
+__device__ __forceinline__ void chain_align_read(const PoaJobDesc &jd, const PoaChainSlot *sl, const PoaChainParams *__restrict__ cp,
+                                                 const PoaParamsDev *__restrict__ prm, const P16Consts &kc, const P16Smem &sm, int ring_rows, int ring_cells,
+                                                 int lane) {
+    PoaJobDesc jp = jd;
+    bool second = false;
+    for (int pass = 0; pass < (STRAND ? 2 : 1); ++pass) {
+        p16_run_job<GAP, GLOBAL, true, false, true>(jp, prm, kc, sm, ring_rows, ring_cells, lane);
+        __syncwarp();
+        if (!STRAND || pass) break;
+        const PoaJobHeader *h = reinterpret_cast<const PoaJobHeader *>(jd.blob);
+        const int qlen = h->qlen;
+        if (jd.result->status != POA_ST_OK || !chain_weak_hit(jd.result->best_score, qlen, h->n_rows, cp->max_mat)) break;
+        const uint8_t *q = sl->reads + sl->read_off[sl->fused];
+        uint8_t *qs = const_cast<uint8_t *>(jd.blob) + h->off_qs;
+        for (int k = lane; k < qlen; k += 32) qs[1 + k] = chain_comp(q[qlen - 1 - k]);
+        __syncwarp();
+        jp.cigar = sl->rc_cigar; jp.result = sl->rc_result;
+        second = true;
+    }
+    if (!STRAND) return;
+    int rc = 0;
+    if (second) {
+        const PoaResultDev *f = jd.result, *b = sl->rc_result;
+        rc = b->status == POA_ST_OK && b->best_score > f->best_score;
+        if (rc) for (int t = lane; t < b->n_ops; t += 32) jd.cigar[t] = sl->rc_cigar[t];
+        __syncwarp();
+        if (lane == 0) {
+            PoaResultDev out = rc ? *b : *f;
+            out.status = f->status != POA_ST_OK ? f->status : b->status;
+            out.cells = f->cells + b->cells; out.fwd_clk = f->fwd_clk + b->fwd_clk; out.bt_clk = f->bt_clk + b->bt_clk;
+            *jd.result = out;
+        }
+    }
+    if (lane == 0) sl->read_rc[sl->fused] = (uint8_t)(rc | (second ? 2 : 0));
+    __syncwarp();
+}
+
 /* ------------------------------------------------------------------ chain engine entry
  * The same job function, fed from device-resident slots (poa_chain.cuh): the job blob of a slot is written
  * by the fuse kernel of the previous round, nothing comes from the host.  Block 0 also zeroes the plane-pool
  * cursor the coming fuse kernel will fill (see PoaChainSlot). */
-template <int GAP>
+template <int GAP, bool STRAND>
 __global__ void POA_P16_BOUNDS poa_chain_align_kernel_p16(const PoaChainSlot *__restrict__ slots, const int32_t *__restrict__ idx,
-                                                           const PoaParamsDev *__restrict__ prm, int n_jobs, int round, int ring_rows, int ring_cells,
-                                                           const __grid_constant__ P16Consts kc) {
+                                                           const PoaChainParams *__restrict__ cp, const PoaParamsDev *__restrict__ prm, int n_jobs,
+                                                           int round, int ring_rows, int ring_cells, const __grid_constant__ P16Consts kc) {
     extern __shared__ __align__(16) uint8_t dyn_smem[];
     const int lane = threadIdx.x;
     const int job = blockIdx.x;
@@ -1812,7 +1860,7 @@ __global__ void POA_P16_BOUNDS poa_chain_align_kernel_p16(const PoaChainSlot *__
     const int n_rows = reinterpret_cast<const PoaJobHeader *>(jd.blob)->n_rows;
     if (sl->failed || sl->fused >= sl->n_reads || n_rows < 3) { if (lane == 0) jd.result->status = POA_ST_SKIP; return; }
     const P16Smem sm = p16_smem_init(dyn_smem, prm, ring_rows, lane);
-    p16_run_job<GAP, GLOBAL, true, false, true>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
+    chain_align_read<GAP, STRAND>(jd, sl, cp, prm, kc, sm, ring_rows, ring_cells, lane);
 }
 
 /* Free-running chain (PoaChainSync in poa_chain.cuh): one resident warp per group runs the group's alignments back to
@@ -1822,9 +1870,10 @@ __device__ __forceinline__ int chain_ld_relaxed(const int32_t *p) { int v; asm v
 __device__ __forceinline__ void chain_st_relaxed(int32_t *p, int v) { asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ unsigned long long chain_now_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
-template <int GAP>
-__global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, PoaChainSync *sync, const PoaParamsDev *__restrict__ prm, int n_groups,
-                                                          int ring_rows, int ring_cells, int dbg, const __grid_constant__ P16Consts kc) {
+template <int GAP, bool STRAND>
+__global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, PoaChainSync *sync, const PoaChainParams *__restrict__ cp,
+                                                          const PoaParamsDev *__restrict__ prm, int n_groups, int ring_rows, int ring_cells, int dbg,
+                                                          const __grid_constant__ P16Consts kc) {
     extern __shared__ __align__(16) uint8_t dyn_smem[];
     const int lane = threadIdx.x;
     const int g = blockIdx.x;
@@ -1861,7 +1910,7 @@ __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, P
         const PoaJobDesc jd = sl->jd;
         const int n_rows = reinterpret_cast<const PoaJobHeader *>(jd.blob)->n_rows;
         if (sl->failed || sl->fused >= sl->n_reads || n_rows < 3) break;
-        p16_run_job<GAP, GLOBAL, true, false, true>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
+        chain_align_read<GAP, STRAND>(jd, sl, cp, prm, kc, sm, ring_rows, ring_cells, lane);
         __syncwarp();
         if (!(dbg & 1)) __threadfence();                       /* release side: CIGAR + result are out before the task is */
         if (lane == 0) {
@@ -1880,50 +1929,62 @@ __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, P
     }
 }
 
-template <int GAP>
-static cudaError_t launch_chain_worker_one(PoaChainSlot *slots, PoaChainSync *sync, int n_groups, const PoaParamsDev *prm, int ring_rows, int ring_cells,
-                                           const P16Consts &kc, cudaStream_t st) {
+template <int GAP, bool STRAND>
+static cudaError_t launch_chain_worker_one(PoaChainSlot *slots, PoaChainSync *sync, int n_groups, const PoaChainParams *cp, const PoaParamsDev *prm,
+                                           int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
     /* at least 23 KB: at most 9 of these CTAs fit one SM, which leaves registers (9 x 160 x 32 of 64 K) and shared memory for a
      * 256-thread fuse worker next to them even if the alignment warps were dispatched first -- they wait for fuse workers */
     /* experiment hooks (timing only): ABPOA_GPU_CHAIN_DBG bit 0 = no fences (UNSAFE), bit 1 = no shared-memory padding; ABPOA_GPU_CHAIN_CARVEOUT */
     static const int dbg = [] { const char *e = getenv("ABPOA_GPU_CHAIN_DBG"); return e && *e ? atoi(e) : 0; }();
     const size_t smem0 = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
     const size_t smem = (dbg & 2) ? smem0 : std::max<size_t>(smem0, (size_t)23 * 1024);
-    cudaError_t e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, STRAND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return e;
     /* the same L1/shared split as the fuse workers ask for (poa_chain.cu): CTAs of both kernels share SMs for the whole run */
     { const char *cv = getenv("ABPOA_GPU_CHAIN_CARVEOUT");
-      e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP>, cudaFuncAttributePreferredSharedMemoryCarveout, cv && *cv ? atoi(cv) : (int)cudaSharedmemCarveoutMaxShared);
+      e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, STRAND>, cudaFuncAttributePreferredSharedMemoryCarveout, cv && *cv ? atoi(cv) : (int)cudaSharedmemCarveoutMaxShared);
       if (e != cudaSuccess) return e; }
-    poa_chain_dp_worker_kernel<GAP><<<n_groups, 32, smem, st>>>(slots, sync, prm, n_groups, ring_rows, ring_cells, dbg, kc);
+    poa_chain_dp_worker_kernel<GAP, STRAND><<<n_groups, 32, smem, st>>>(slots, sync, cp, prm, n_groups, ring_rows, ring_cells, dbg, kc);
     return cudaGetLastError();
 }
+/* strand: the host's PoaChainParams::amb_strand (-s), which picks the kernel instantiation */
 extern "C" cudaError_t poa_launch_chain_dp_worker(int gap_mode, const int *gaps, PoaChainSlot *slots, PoaChainSync *sync, int n_groups,
-                                                  const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st) {
+                                                  const PoaChainParams *cp, int strand, const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st) {
     if (n_groups <= 0) return cudaSuccess;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    if (gap_mode == LG) return launch_chain_worker_one<LG>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st);
-    if (gap_mode == AG) return launch_chain_worker_one<AG>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st);
-    return launch_chain_worker_one<CG>(slots, sync, n_groups, prm, ring_rows, ring_cells, kc, st);
+    if (strand) {
+        if (gap_mode == LG) return launch_chain_worker_one<LG, true>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+        if (gap_mode == AG) return launch_chain_worker_one<AG, true>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+        return launch_chain_worker_one<CG, true>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    }
+    if (gap_mode == LG) return launch_chain_worker_one<LG, false>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == AG) return launch_chain_worker_one<AG, false>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    return launch_chain_worker_one<CG, false>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
 }
 
-template <int GAP>
-static cudaError_t launch_chain_one(const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round, const PoaParamsDev *prm, int ring_rows, int ring_cells,
-                                    const P16Consts &kc, cudaStream_t st) {
+template <int GAP, bool STRAND>
+static cudaError_t launch_chain_one(const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round, const PoaChainParams *cp, const PoaParamsDev *prm,
+                                    int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
     const size_t smem = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
-    cudaError_t e = cudaFuncSetAttribute(poa_chain_align_kernel_p16<GAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_align_kernel_p16<GAP, STRAND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return e;
-    poa_chain_align_kernel_p16<GAP><<<n_jobs, 32, smem, st>>>(slots, idx, prm, n_jobs, round, ring_rows, ring_cells, kc);
+    poa_chain_align_kernel_p16<GAP, STRAND><<<n_jobs, 32, smem, st>>>(slots, idx, cp, prm, n_jobs, round, ring_rows, ring_cells, kc);
     return cudaGetLastError();
 }
 /* gaps[4] = { e1, oe1, e2, oe2 } (host copy of what prm holds on the device) */
 extern "C" cudaError_t poa_launch_chain_align_p16(int gap_mode, const int *gaps, const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round,
-                                                  const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st) {
+                                                  const PoaChainParams *cp, int strand, const PoaParamsDev *prm, int ring_rows, int ring_cells,
+                                                  cudaStream_t st) {
     if (n_jobs <= 0) return cudaSuccess;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    if (gap_mode == LG) return launch_chain_one<LG>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
-    if (gap_mode == AG) return launch_chain_one<AG>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
-    return launch_chain_one<CG>(slots, idx, n_jobs, round, prm, ring_rows, ring_cells, kc, st);
+    if (strand) {
+        if (gap_mode == LG) return launch_chain_one<LG, true>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+        if (gap_mode == AG) return launch_chain_one<AG, true>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+        return launch_chain_one<CG, true>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    }
+    if (gap_mode == LG) return launch_chain_one<LG, false>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == AG) return launch_chain_one<AG, false>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    return launch_chain_one<CG, false>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
 }
 
 /* ------------------------------------------------------------------ debug: the chain's job function on one job

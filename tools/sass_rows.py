@@ -85,13 +85,13 @@ def disassemble(src: Path, tmp: Path, gap: int):
     cubin = tmp / "k.cubin"
     subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
                     f"-I{ROOT / 'include'}", f"-I{ROOT / 'abpoa_b200' / 'csrc'}", "-cubin", "-o", str(cubin), str(src)], check=True)
-    fn = f"_Z26poa_chain_dp_worker_kernelILi{gap}EEvP12PoaChainSlotP12PoaChainSyncPK12PoaParamsDeviiii9P16Consts"
     res = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-res-usage", str(cubin)], check=True, capture_output=True, text=True).stdout
+    fn = re.search(rf"Function (_Z26poa_chain_dp_worker_kernelILi{gap}E(?:Lb0E)?Ev\w+):", res).group(1)     # without -s
     m = re.search(re.escape(fn) + r":\s*\n\s*REG:(\d+)", res)
     regs = int(m.group(1)) if m else None
     dis = subprocess.run(["/usr/local/cuda/bin/nvdisasm", "-gi", str(cubin)], check=True, capture_output=True, text=True).stdout
     a = dis.index(f".text.{fn}:")
-    b = dis.find("\n.section", a + 1)
+    b = min((k for k in (dis.find("\n.section", a + 1), dis.find("\n\t.section", a + 1)) if k > 0), default=-1)
     return dis[a: b if b > 0 else None].splitlines(), regs
 
 
