@@ -96,7 +96,8 @@ class PackedGroups:
     """Host-side argument block for abpoa_gpu_msa_batch (keeps the numpy buffers alive)."""
 
     def __init__(self, groups: Sequence[Sequence[np.ndarray]], weights=None):
-        """weights: optional per group list of per-read int32 base weights (the reference's -Q), or None."""
+        """weights: optional per group list of per-read int32 base weights (the reference's -Q; None for a read without
+        them: unit weights), or None."""
         self.n = len(groups)
         self._keep = []
         self.arr = (abpoa_gpu_group_t * self.n)()
@@ -113,8 +114,8 @@ class PackedGroups:
             self.arr[g].seqs = C.cast(ptrs, C.POINTER(c_u8_p))
             self.arr[g].qual_weights = None
             if weights is not None and weights[g] is not None:
-                ws = [np.ascontiguousarray(w, dtype=np.int32) for w in weights[g]]
-                wp = (c_int_p * n)(*[w.ctypes.data_as(c_int_p) for w in ws])
+                ws = [None if w is None else np.ascontiguousarray(w, dtype=np.int32) for w in weights[g]]
+                wp = (c_int_p * n)(*[None if w is None else w.ctypes.data_as(c_int_p) for w in ws])
                 self._keep += [ws, wp]
                 self.arr[g].qual_weights = C.cast(wp, C.POINTER(c_int_p))
             self.total_bases += sum(len(a) for a in arrs)

@@ -28,8 +28,9 @@
  *
  * Scope of the chain: global alignment, banded (wb >= 0), packed-int16 admissible scores, heaviest-bundling or
  * most-frequent-base consensus (single cluster, no sub_aln), row-column MSA and GFA (one read set per node, not per
- * edge), unit base weights, ambiguous strand (-s: the alignment warp retries a weak hit as the reverse complement,
- * chain_align_read in poa_kernels.cu).  Everything else takes the other engine.
+ * edge), base weights (-Q: a weight byte per read base, 0..255; a group with any other weight takes the other engine),
+ * ambiguous strand (-s: the alignment warp retries a weak hit as the reverse complement, chain_align_read in
+ * poa_kernels.cu).  Everything else takes the other engine.
  */
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -246,7 +247,7 @@ int poa_chain_eligible(const abpoa_para_t *abpt) {
     const int mf = abpt->cons_algrm == ABPOA_MF && abpt->use_read_ids && !abpt->sub_aln;
     if (abpt->cons_algrm != ABPOA_HB && !mf) return 0;
     if ((abpt->use_read_ids && !abpt->out_msa && !abpt->out_gfa && !mf) || abpt->max_n_cons > 1) return 0;
-    if (abpt->use_qv || abpt->inc_path_score || abpt->zdrop > 0 || abpt->rev_cigar || !abpt->ret_cigar) return 0;
+    if (abpt->inc_path_score || abpt->zdrop > 0 || abpt->rev_cigar || !abpt->ret_cigar) return 0;
     if (abpt->put_gap_on_right || abpt->put_gap_at_end) return 0;         /* handled by the kernels, but keep the chain on the common configuration */
     if (abpt->m > POA_MAX_M) return 0;
     if (!(abpt->disable_seeding && abpt->progressive_poa == 0)) return 0;
@@ -342,6 +343,7 @@ struct ChainCall {
     int W;                  /* RC-MSA / GFA: words per read set (W of the largest group), 0 otherwise */
     bool export_graph;      /* the whole graph comes back (compact export) and the host computes the consensus on it */
     bool strand;            /* -s: the alignment warp retries weak hits as the reverse complement; read_rc comes back */
+    bool qv;                /* -Q and at least one read with weights: every group gets its weight bytes (chain_slot_reads) */
     int sm_count;
 };
 
@@ -364,6 +366,10 @@ ChainCall chain_call(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_worker
     c.with_cons = abpt->out_cons ? 1 : 0;
     c.mf = abpt->cons_algrm == ABPOA_MF;
     c.strand = abpt->amb_strand != 0;
+    c.qv = false;
+    if (abpt->use_qv)
+        for (int g : todo)
+            for (int i = 0; groups[g].qual_weights && i < groups[g].n_seq && !c.qv; ++i) c.qv = groups[g].qual_weights[i] != NULL;
     c.W = 0;
     if (c.want_msa || c.want_gfa) for (int g : todo) c.W = std::max(c.W, (groups[g].n_seq + 63) / 64);
     c.sm_count = 132;
@@ -384,6 +390,9 @@ std::vector<GroupPlan> plan_groups(const ChainCall &c, const std::vector<int> &t
             if (l > p.qmax) p.qmax = l;
             p.bases += l;
             if (ok && !poa_p16_ok(c.abpt, l, 3 * l)) ok = false;
+            /* the device keeps one byte per weight: a group with any other weight is finished by the launch engine */
+            const int *qw = c.qv && in.qual_weights ? in.qual_weights[i] : NULL;
+            for (int j = 0; ok && qw && j < l; ++j) ok = qw[j] >= 0 && qw[j] <= 255;
         }
         if (!ok || p.qmax > (1 << 24)) { fallback.push_back(g); continue; }
         /* node capacity: 10 % growth per read, and for large groups at most 4 % plus a fixed slack (5 % error, 50 x 10 kbp:
@@ -395,7 +404,7 @@ std::vector<GroupPlan> plan_groups(const ChainCall &c, const std::vector<int> &t
         PoaChainSlot probe;
         size_t own = 0; p.reads_bytes = 0;
         chain_slot_layout(&probe, p.n_cap, p.qmax, p.n_reads, c.K, c.A, c.m, c.W, c.record, [&](size_t b) { own += al256(b); return (uint8_t *)NULL; }, c.strand);
-        chain_slot_reads(&probe, p.n_reads, p.bases, [&](size_t b) { p.reads_bytes += al256(b); return (uint8_t *)NULL; });
+        chain_slot_reads(&probe, p.n_reads, p.bases, [&](size_t b) { p.reads_bytes += al256(b); return (uint8_t *)NULL; }, c.qv);
         p.static_bytes = own + p.reads_bytes;
         const size_t nc = (size_t)p.n_cap;
         /* result records in the (then idle) plane pool: consensus + MSA rows, msa_len <= nodes */
@@ -550,7 +559,7 @@ struct Wave {
             const abpoa_gpu_group_t &in = c.groups[p.g];
             PoaChainSlot &s = hs[t]; memset(&s, 0, sizeof s);
             chain_slot_layout(&s, p.n_cap, p.qmax, p.n_reads, c.K, c.A, c.m, c.W, c.record, gtake, c.strand);
-            chain_slot_reads(&s, p.n_reads, p.bases, rtake);
+            chain_slot_reads(&s, p.n_reads, p.bases, rtake, c.qv);
             int32_t *hoff = (int32_t *)(h_reads + ((const uint8_t *)s.read_off - d_reads)), *hw = (int32_t *)(h_reads + ((const uint8_t *)s.read_w - d_reads));
             int acc = 0;
             for (int i = 0; i < p.n_reads; ++i) {
@@ -561,7 +570,8 @@ struct Wave {
             }
             hoff[p.n_reads] = acc;
         }
-        /* the read bytes themselves: half a gigabyte at BASELINE size, copied into the pinned buffer by all workers */
+        /* the read bytes themselves: half a gigabyte at BASELINE size, copied into the pinned buffer by all workers; -Q: the
+         * weights too (plan_groups checked that they fit a byte), 1 for a read without them */
         {
             std::atomic<int> nx(0);
             auto copy_reads = [&]() {
@@ -569,6 +579,14 @@ struct Wave {
                     const abpoa_gpu_group_t &in = c.groups[plans[t].g];
                     uint8_t *q = h_reads + (hs[t].reads - d_reads);
                     for (int i = 0; i < in.n_seq; ++i) { memcpy(q, in.seqs[i], (size_t)in.seq_lens[i]); q += in.seq_lens[i]; }
+                    if (!c.qv) continue;
+                    uint8_t *w = h_reads + (hs[t].read_qw - d_reads);
+                    for (int i = 0; i < in.n_seq; ++i) {
+                        const int *qw = in.qual_weights ? in.qual_weights[i] : NULL;
+                        if (qw) for (int j = 0; j < in.seq_lens[i]; ++j) w[j] = (uint8_t)qw[j];
+                        else memset(w, 1, (size_t)in.seq_lens[i]);
+                        w += in.seq_lens[i];
+                    }
                 }
             };
             const int nth = reads_bytes < (8u << 20) ? 1 : std::max(1, std::min(c.n_workers, 16));

@@ -112,6 +112,9 @@ typedef struct PoaChainSlot {           /* one per read group; every pointer aim
     uint8_t *read_rc;                                   /* [n_reads] */
     uint64_t *rc_cigar;                                 /* [jd.cigar_cap] */
     PoaResultDev *rc_result;
+    /* -Q (use_qv): the weight of every read base (the edge that enters the base's node gets it), at the reads' offsets;
+     * NULL: unit weights */
+    const uint8_t *read_qw;                             /* [sum of the read lengths] */
 } PoaChainSlot;
 
 /* A group's memory, host side: the slot's capacities and every per-group array, taken in one fixed order from the
@@ -147,12 +150,14 @@ static inline void chain_slot_layout(PoaChainSlot *s, int n_cap, int qmax, int n
     }
 }
 
-/* the group's reads: `bases` bytes back to back, n_reads + 1 offsets, n_reads band half widths */
+/* the group's reads: `bases` bytes back to back, n_reads + 1 offsets, n_reads band half widths; `qv` (-Q runs with
+ * weights) adds one weight byte per base behind them */
 template <class Take>
-static inline void chain_slot_reads(PoaChainSlot *s, int n_reads, int64_t bases, Take take) {
+static inline void chain_slot_reads(PoaChainSlot *s, int n_reads, int64_t bases, Take take, bool qv = false) {
     s->reads = (const uint8_t *)take((size_t)bases);
     s->read_off = (const int32_t *)take(((size_t)n_reads + 1) * 4);
     s->read_w = (const int32_t *)take((size_t)n_reads * 4);
+    if (qv) s->read_qw = (const uint8_t *)take((size_t)bases);
 }
 
 /* Free-running chain: every group advances at its own pace.  One resident warp per group runs its alignments back to back;
@@ -286,12 +291,23 @@ POA_DEV bool chain_weak_hit(int best_score, int qlen, int node_n, int max_mat) {
 /* complement of a base code (reference src/abpoa_align.c:329): 0..3 -> 3..0, everything else -> 4, with -c too */
 POA_DEV uint8_t chain_comp(uint8_t b) { return b < 4 ? (uint8_t)(3 - b) : (uint8_t)4; }
 
-/* base qi of read r on the strand it is fused on: the reverse complement, computed on the fly, when read_rc[r] says so */
-POA_DEV uint8_t chain_read_base(const PoaChainSlot *s, int r, int qi) {
-    const uint8_t *q = s->reads + s->read_off[r];
-    if (s->read_rc && (s->read_rc[r] & 1)) return chain_comp(q[s->read_off[r + 1] - s->read_off[r] - 1 - qi]);
-    return q[qi];
+/* read r as the graph code fuses it, looked up once per read: its bases, its -Q weights (NULL: unit weights), its length
+ * and whether it is fused as the reverse complement (read_rc[r]) */
+typedef struct ChainRead { const uint8_t *q, *w; int len; bool rc; } ChainRead;
+
+POA_DEV ChainRead chain_read(const PoaChainSlot *s, int r) {
+    ChainRead rd;
+    rd.q = s->reads + s->read_off[r]; rd.w = s->read_qw ? s->read_qw + s->read_off[r] : NULL;
+    rd.len = s->read_off[r + 1] - s->read_off[r]; rd.rc = s->read_rc && (s->read_rc[r] & 1);
+    return rd;
 }
+
+/* base qi on the strand the read is fused on: the reverse complement, computed on the fly */
+POA_DEV uint8_t chain_read_base(const ChainRead &rd, int qi) { return rd.rc ? chain_comp(rd.q[rd.len - 1 - qi]) : rd.q[qi]; }
+
+/* -Q: weight of base qi on the strand the read is fused on (a reverse-complemented read's weights are reversed, as in
+ * poa_msa.c and the launch engine), 1 without weights */
+POA_DEV int chain_read_weight(const ChainRead &rd, int qi) { return !rd.w ? 1 : rd.w[rd.rc ? rd.len - 1 - qi : qi]; }
 
 /* ------------------------------------------------------------------ order-dependent passes */
 /* max_remain by row: remain[row] = remain[row of heaviest out-neighbour] + 1, SINK = -1 (reference
@@ -403,11 +419,14 @@ POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int3
 }
 
 /* ------------------------------------------------------------------ first read of a group */
-/* a chain SRC -> b0 -> b1 ... -> SINK (reference src/abpoa_graph.c:573-593) */
+/* a chain SRC -> b0 -> b1 ... -> SINK (reference src/abpoa_graph.c:573-593): the edge into b_i weighs w[i], the edge into
+ * SINK w[len - 1] */
 POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
     const int K = cp->K;
-    const int len = s->read_off[1] - s->read_off[0];
-    const uint8_t *q = s->reads + s->read_off[0];
+    ChainRead rd = chain_read(s, 0);
+    rd.rc = false;                                       /* read 0 is fused forward (its strand byte is cleared below) */
+    const int len = rd.len;
+    const uint8_t *q = rd.q;
     const int n = len + 2;
     if (n > s->n_cap || len < 1) {
         if (POA_TID0) { POA_ATOMIC_OR(&s->failed, POA_CF_NODE_CAP); reinterpret_cast<PoaJobHeader *>(const_cast<uint8_t *>(s->jd.blob))->n_rows = 0; }
@@ -418,15 +437,15 @@ POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
     POA_PAR_FOR(v, n) {
         /* node ids: 0 SRC, 1 SINK, 2 + i = base i */
         s->aln_cnt[v] = 0;
-        if (v == 0) { s->base[v] = 0; s->in_cnt[v] = 0; s->out_cnt[v] = 1; s->out_id[0] = 2; s->out_w[0] = 1; s->n_read[v] = 1; order[0] = 0; s->node_row[0] = 0; }
+        if (v == 0) { s->base[v] = 0; s->in_cnt[v] = 0; s->out_cnt[v] = 1; s->out_id[0] = 2; s->out_w[0] = chain_read_weight(rd, 0); s->n_read[v] = 1; order[0] = 0; s->node_row[0] = 0; }
         else if (v == 1) {
-            s->base[v] = 0; s->out_cnt[v] = 0; s->in_cnt[v] = 1; s->in_id[(size_t)K] = len + 1; s->in_w[(size_t)K] = 1; s->n_read[v] = 0;
+            s->base[v] = 0; s->out_cnt[v] = 0; s->in_cnt[v] = 1; s->in_id[(size_t)K] = len + 1; s->in_w[(size_t)K] = chain_read_weight(rd, len - 1); s->n_read[v] = 0;
             order[n - 1] = 1; s->node_row[1] = n - 1;
         } else {
             const int i = v - 2;
             s->base[v] = q[i];
-            s->in_cnt[v] = 1; s->in_id[(size_t)v * K] = i == 0 ? 0 : v - 1; s->in_w[(size_t)v * K] = 1;
-            s->out_cnt[v] = 1; s->out_id[(size_t)v * K] = i == len - 1 ? 1 : v + 1; s->out_w[(size_t)v * K] = 1;
+            s->in_cnt[v] = 1; s->in_id[(size_t)v * K] = i == 0 ? 0 : v - 1; s->in_w[(size_t)v * K] = chain_read_weight(rd, i);
+            s->out_cnt[v] = 1; s->out_id[(size_t)v * K] = i == len - 1 ? 1 : v + 1; s->out_w[(size_t)v * K] = chain_read_weight(rd, i == len - 1 ? i : i + 1);
             s->n_read[v] = 1;
             order[i + 1] = v; s->node_row[v] = i + 1;
         }
@@ -467,7 +486,8 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
         POA_CTA_SYNC();
         return;
     }
-    const int qlen = s->read_off[r + 1] - s->read_off[r];
+    const ChainRead rd = chain_read(s, r);
+    const int qlen = rd.len;
     const uint64_t *ops = s->jd.cigar;
     const int n_ops = res->n_ops;
     const int old_n = s->n_nodes;
@@ -518,7 +538,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
         if (row == -2) POA_ATOMIC_OR(&s->failed, POA_CF_CIGAR);          /* global mode: every base is M or I */
         if (row >= 0) {
             const int v = order[row];
-            const uint8_t b = chain_read_base(s, r, qi);
+            const uint8_t b = chain_read_base(rd, qi);
             if (s->base[v] == b) { kind = CK_OLD; target = v; }
             else {
                 const int na = s->aln_cnt[v]; const int32_t *al = s->aln_id + (size_t)v * A;
@@ -575,7 +595,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
         if (isnew[qi]) {
             const int id = old_n + newidx[qi];
             const int col = tgt[qi];                         /* CK_NEWM: the column's node */
-            s->base[id] = chain_read_base(s, r, qi); s->in_cnt[id] = 0; s->out_cnt[id] = 0; s->aln_cnt[id] = 0; s->n_read[id] = 0;
+            s->base[id] = chain_read_base(rd, qi); s->in_cnt[id] = 0; s->out_cnt[id] = 0; s->aln_cnt[id] = 0; s->n_read[id] = 0;
             if (cp->W > 0) for (int wd = 0; wd < cp->W; ++wd) s->read_set[(size_t)id * cp->W + wd] = 0;
             new_anchor[newidx[qi]] = kind_anchor[qi] & 0x0fffffff;      /* compacted: by new-node rank (anchors are non-decreasing) */
             item_row[qi] = col;                              /* remember the column for the aligned-set update */
@@ -585,11 +605,12 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
     POA_CTA_SYNC();
     /* new_anchor was written by rank while being read by item in the loop above only through kind_anchor: safe */
 
-    /* ---- 6. edges: item qi owns in-list(tgt[qi]) and out-list(tgt[qi-1]); item qlen is the closing edge to SINK ---- */
+    /* ---- 6. edges: item qi owns in-list(tgt[qi]) and out-list(tgt[qi-1]); item qlen is the closing edge to SINK.
+     *         Weights (-Q) add to the edges; n_read counts reads ---- */
     POA_PAR_FOR(qi, qlen + 1) {
         const int from = qi == 0 ? 0 : tgt[qi - 1], to = qi < qlen ? tgt[qi] : 1;
         const int from_new = qi > 0 && isnew[qi - 1], to_new = qi < qlen && isnew[qi];
-        const int w = 1;
+        const int w = chain_read_weight(rd, qi < qlen ? qi : qlen - 1);       /* the closing edge: the last base's */
         int32_t *iid = s->in_id + (size_t)to * K, *iw = s->in_w + (size_t)to * K;
         int32_t *oid = s->out_id + (size_t)from * K, *ow = s->out_w + (size_t)from * K;
         int nin = s->in_cnt[to], nout = s->out_cnt[from];
