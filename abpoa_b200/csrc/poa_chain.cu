@@ -30,7 +30,8 @@
  * most-frequent-base consensus (single cluster, no sub_aln), row-column MSA and GFA (one read set per node, not per
  * edge), base weights (-Q: a weight byte per read base, 0..255; a group with any other weight takes the other engine),
  * ambiguous strand (-s: the alignment warp retries a weak hit as the reverse complement, chain_align_read in
- * poa_kernels.cu).  Everything else takes the other engine.
+ * poa_kernels.cu), path scores (-G: the flatten writes every in-edge's score, chain_path_score; a group whose node weights
+ * could exceed POA_PS_MAX_NODE_W takes the other engine).  Everything else takes the other engine.
  */
 #include <cuda_runtime.h>
 #include <algorithm>
@@ -55,9 +56,11 @@
     poa_die("libabpoa_b200/chain", "%s failed at %s:%d: %s", #call, __FILE__, __LINE__, cudaGetErrorString(e_)); } while (0)
 
 extern "C" cudaError_t poa_launch_chain_dp_worker(int gap_mode, const int *gaps, PoaChainSlot *slots, PoaChainSync *sync, int n_groups,
-                                                  const PoaChainParams *cp, int strand, const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st);
+                                                  const PoaChainParams *cp, int strand, int ps, const PoaParamsDev *prm, int ring_rows, int ring_cells,
+                                                  cudaStream_t st);
 extern "C" cudaError_t poa_launch_chain_align_p16(int gap_mode, const int *gaps, const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round,
-                                                  const PoaChainParams *cp, int strand, const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st);
+                                                  const PoaChainParams *cp, int strand, int ps, const PoaParamsDev *prm, int ring_rows, int ring_cells,
+                                                  cudaStream_t st);
 extern "C" void poa_pick_ring(int gap_mode, int bits, int band_cells, size_t smem_budget, int *ring_rows, int *ring_cells);
 
 static_assert(offsetof(PoaChainSync, q_tail) == 128 && offsetof(PoaChainSync, total) == 256 && offsetof(PoaChainSync, abort) == 384,
@@ -65,14 +68,17 @@ static_assert(offsetof(PoaChainSync, q_tail) == 128 && offsetof(PoaChainSync, to
 static_assert(POA_GFA_HDR_WORDS == POA_GFA_HDR, "the device's GFA record header is the one poa_gfa_from_record reads");
 
 /* ------------------------------------------------------------------ kernels */
+/* PS: -G runs (ChainCall::ps), whose jobs carry path scores (chain_flatten) */
+template <bool PS>
 __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_seed_kernel(PoaChainSlot *slots, const PoaChainParams *cp, int n) {
     if ((int)blockIdx.x >= n) return;
-    chain_seed(&slots[blockIdx.x], cp);
+    chain_seed<PS>(&slots[blockIdx.x], cp);
 }
 
+template <bool PS>
 __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_fuse_kernel(PoaChainSlot *slots, const int32_t *idx, const PoaChainParams *cp, int n, int round) {
     if ((int)blockIdx.x >= n) return;
-    chain_fuse(&slots[idx[blockIdx.x]], cp, round);
+    chain_fuse<PS>(&slots[idx[blockIdx.x]], cp, round);
 }
 
 /* Free-running chain, fuse side: persistent CTAs draw tickets from PoaChainSync; ticket t is served when tasks[t] holds a group.
@@ -81,6 +87,7 @@ __device__ __forceinline__ int sync_ld(const int32_t *p) { int v; asm volatile("
 __device__ __forceinline__ void sync_st(int32_t *p, int v) { asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ unsigned long long sync_now_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
+template <bool PS>
 __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_fuse_worker_kernel(PoaChainSlot *slots, PoaChainSync *sync, const PoaChainParams *cp) {
     __shared__ int task_s;
     for (;;) {
@@ -114,7 +121,7 @@ __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_fuse_worker_kernel(PoaC
         __threadfence();                                       /* acquire: graph arrays / CIGAR of this group may have been written from another SM */
         PoaChainSlot *s = &slots[g];
         const unsigned long long t0 = sync_now_ns();
-        chain_fuse(s, cp, 0);
+        chain_fuse<PS>(s, cp, 0);
         __syncthreads();
         __threadfence();                                       /* release */
         __syncthreads();
@@ -232,8 +239,28 @@ __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_gfa_kernel(PoaChainSlot
     chain_gfa_record(s, cp, hdr_s, out + at_s);
 }
 
+/* debugging aid (tests): the device's -G score function on n (edge weight, node weight) pairs */
+__global__ void poa_chain_path_score_kernel(const int32_t *edge_w, const int32_t *node_w, int n, int32_t *out) {
+    for (int i = (int)(blockIdx.x * blockDim.x + threadIdx.x); i < n; i += (int)(gridDim.x * blockDim.x)) out[i] = chain_path_score(edge_w[i], node_w[i]);
+}
+
 /* ------------------------------------------------------------------ host side */
 static inline size_t al256(size_t x) { return (x + 255) & ~(size_t)255; }
+
+/* debugging aid (tests): out[i] = chain_path_score(edge_w[i], node_w[i]) computed on the current device */
+extern "C" int poa_debug_path_scores(const int32_t *edge_w, const int32_t *node_w, int n, int32_t *out) {
+    if (n <= 0) return 0;
+    int32_t *d = NULL;
+    const size_t b = (size_t)n * 4;
+    CK(cudaMalloc((void **)&d, 3 * b));
+    CK(cudaMemcpy(d, edge_w, b, cudaMemcpyHostToDevice));
+    CK(cudaMemcpy(d + n, node_w, b, cudaMemcpyHostToDevice));
+    poa_chain_path_score_kernel<<<(n + 255) / 256 < 4096 ? (n + 255) / 256 : 4096, 256>>>(d, d + n, n, d + 2 * (size_t)n);
+    CK(cudaGetLastError());
+    CK(cudaMemcpy(out, d + 2 * (size_t)n, b, cudaMemcpyDeviceToHost));
+    CK(cudaFree(d));
+    return n;
+}
 
 int poa_chain_eligible(const abpoa_para_t *abpt) {
     const char *off = getenv("ABPOA_GPU_NO_CHAIN");
@@ -247,7 +274,7 @@ int poa_chain_eligible(const abpoa_para_t *abpt) {
     const int mf = abpt->cons_algrm == ABPOA_MF && abpt->use_read_ids && !abpt->sub_aln;
     if (abpt->cons_algrm != ABPOA_HB && !mf) return 0;
     if ((abpt->use_read_ids && !abpt->out_msa && !abpt->out_gfa && !mf) || abpt->max_n_cons > 1) return 0;
-    if (abpt->inc_path_score || abpt->zdrop > 0 || abpt->rev_cigar || !abpt->ret_cigar) return 0;
+    if (abpt->zdrop > 0 || abpt->rev_cigar || !abpt->ret_cigar) return 0;
     if (abpt->put_gap_on_right || abpt->put_gap_at_end) return 0;         /* handled by the kernels, but keep the chain on the common configuration */
     if (abpt->m > POA_MAX_M) return 0;
     if (!(abpt->disable_seeding && abpt->progressive_poa == 0)) return 0;
@@ -344,6 +371,7 @@ struct ChainCall {
     bool export_graph;      /* the whole graph comes back (compact export) and the host computes the consensus on it */
     bool strand;            /* -s: the alignment warp retries weak hits as the reverse complement; read_rc comes back */
     bool qv;                /* -Q and at least one read with weights: every group gets its weight bytes (chain_slot_reads) */
+    bool ps;                /* -G: every job blob carries path scores; the kernels' path-score instantiation runs */
     int sm_count;
 };
 
@@ -366,6 +394,7 @@ ChainCall chain_call(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_worker
     c.with_cons = abpt->out_cons ? 1 : 0;
     c.mf = abpt->cons_algrm == ABPOA_MF;
     c.strand = abpt->amb_strand != 0;
+    c.ps = abpt->inc_path_score != 0;
     c.qv = false;
     if (abpt->use_qv)
         for (int g : todo)
@@ -394,6 +423,9 @@ std::vector<GroupPlan> plan_groups(const ChainCall &c, const std::vector<int> &t
             const int *qw = c.qv && in.qual_weights ? in.qual_weights[i] : NULL;
             for (int j = 0; ok && qw && j < l; ++j) ok = qw[j] >= 0 && qw[j] <= 255;
         }
+        /* -G: a node weighs at most n_reads x the largest weight; past POA_PS_MAX_NODE_W the device's log is not known to round
+         * as the host's does */
+        if (c.ps && (int64_t)in.n_seq * (c.qv ? 255 : 1) > POA_PS_MAX_NODE_W) ok = false;
         if (!ok || p.qmax > (1 << 24)) { fallback.push_back(g); continue; }
         /* node capacity: 10 % growth per read, and for large groups at most 4 % plus a fixed slack (5 % error, 50 x 10 kbp:
          * 3.0 % measured, 33.8k nodes reserved for 25k used) -- a group that outgrows it goes to the launch engine */
@@ -403,7 +435,7 @@ std::vector<GroupPlan> plan_groups(const ChainCall &c, const std::vector<int> &t
         /* what the wave carve will take for the group, at its 256-byte granularity */
         PoaChainSlot probe;
         size_t own = 0; p.reads_bytes = 0;
-        chain_slot_layout(&probe, p.n_cap, p.qmax, p.n_reads, c.K, c.A, c.m, c.W, c.record, [&](size_t b) { own += al256(b); return (uint8_t *)NULL; }, c.strand);
+        chain_slot_layout(&probe, p.n_cap, p.qmax, p.n_reads, c.K, c.A, c.m, c.W, c.record, [&](size_t b) { own += al256(b); return (uint8_t *)NULL; }, c.strand, c.ps);
         chain_slot_reads(&probe, p.n_reads, p.bases, [&](size_t b) { p.reads_bytes += al256(b); return (uint8_t *)NULL; }, c.qv);
         p.static_bytes = own + p.reads_bytes;
         const size_t nc = (size_t)p.n_cap;
@@ -558,7 +590,7 @@ struct Wave {
             const GroupPlan &p = plans[t];
             const abpoa_gpu_group_t &in = c.groups[p.g];
             PoaChainSlot &s = hs[t]; memset(&s, 0, sizeof s);
-            chain_slot_layout(&s, p.n_cap, p.qmax, p.n_reads, c.K, c.A, c.m, c.W, c.record, gtake, c.strand);
+            chain_slot_layout(&s, p.n_cap, p.qmax, p.n_reads, c.K, c.A, c.m, c.W, c.record, gtake, c.strand, c.ps);
             chain_slot_reads(&s, p.n_reads, p.bases, rtake, c.qv);
             int32_t *hoff = (int32_t *)(h_reads + ((const uint8_t *)s.read_off - d_reads)), *hw = (int32_t *)(h_reads + ((const uint8_t *)s.read_w - d_reads));
             int acc = 0;
@@ -643,7 +675,8 @@ struct Wave {
         h2d = reads_bytes + (uint64_t)nw * sizeof(PoaChainSlot) + sizeof hcp + sizeof hprm + idx.size() * 4 + (uint64_t)nw * 12;
         /* timed region of the device work: inputs are resident when ev_t0 fires */
         CK(cudaEventRecord(ev_t0, s0));
-        poa_chain_seed_kernel<<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw);
+        if (c.ps) poa_chain_seed_kernel<true><<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw);
+        else poa_chain_seed_kernel<false><<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw);
         CK(cudaGetLastError());
         CK(cudaEventRecord(ev_up, s0));
         static const size_t smem_budget = [] { const char *e = getenv("ABPOA_GPU_SMEM_KB"); return (size_t)(e && *e ? atoi(e) : 28) * 1024; }();
@@ -689,13 +722,15 @@ struct Wave {
          * with one fuse CTA on every SM (default split of a 5 KB kernel: 64 KB) the alignment grid (split: maximum) never
          * started, and neither kernel ever ends by itself (measured: the fuse workers' watchdog fired, then the alignment
          * grid ran). */
-        CK(cudaFuncSetAttribute(poa_chain_fuse_worker_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+        CK(cudaFuncSetAttribute(c.ps ? poa_chain_fuse_worker_kernel<true> : poa_chain_fuse_worker_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                cudaSharedmemCarveoutMaxShared));
         static const bool dp_first = [] { const char *e = getenv("ABPOA_GPU_CHAIN_DP_FIRST"); return e && *e == '1'; }();     /* experiment */
         CK(cudaStreamWaitEvent(st_dp, ev_sync, 0));
-        if (dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, d_prm, ring_rows, ring_cells, st_dp));
-        poa_chain_fuse_worker_kernel<<<n_fuse, POA_CHAIN_T, 0, s0>>>(d_slots, d_sync, d_cp);
+        if (dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, c.ps, d_prm, ring_rows, ring_cells, st_dp));
+        if (c.ps) poa_chain_fuse_worker_kernel<true><<<n_fuse, POA_CHAIN_T, 0, s0>>>(d_slots, d_sync, d_cp);
+        else poa_chain_fuse_worker_kernel<false><<<n_fuse, POA_CHAIN_T, 0, s0>>>(d_slots, d_sync, d_cp);
         CK(cudaGetLastError());
-        if (!dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, d_prm, ring_rows, ring_cells, st_dp));
+        if (!dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, c.ps, d_prm, ring_rows, ring_cells, st_dp));
         cudaEvent_t ev_dp; CK(cudaEventCreateWithFlags(&ev_dp, cudaEventDisableTiming));
         CK(cudaEventRecord(ev_dp, st_dp));
         CK(cudaStreamWaitEvent(s0, ev_dp, 0));
@@ -742,9 +777,10 @@ struct Wave {
                 cudaEvent_t e0, e1, e2; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1)); CK(cudaEventCreate(&e2));
                 coh[k].marks.push_back(e0); coh[k].marks.push_back(e1); coh[k].marks.push_back(e2);
                 CK(cudaEventRecord(e0, st));
-                CK(poa_launch_chain_align_p16(c.abpt->gap_mode, gaps, d_slots, d_idx + ro.first, ro.second, r, d_cp, c.strand, d_prm, ring_rows, ring_cells, st));
+                CK(poa_launch_chain_align_p16(c.abpt->gap_mode, gaps, d_slots, d_idx + ro.first, ro.second, r, d_cp, c.strand, c.ps, d_prm, ring_rows, ring_cells, st));
                 CK(cudaEventRecord(e1, st));
-                poa_chain_fuse_kernel<<<ro.second, POA_CHAIN_T, 0, st>>>(d_slots, d_idx + ro.first, d_cp, ro.second, r);
+                if (c.ps) poa_chain_fuse_kernel<true><<<ro.second, POA_CHAIN_T, 0, st>>>(d_slots, d_idx + ro.first, d_cp, ro.second, r);
+                else poa_chain_fuse_kernel<false><<<ro.second, POA_CHAIN_T, 0, st>>>(d_slots, d_idx + ro.first, d_cp, ro.second, r);
                 CK(cudaGetLastError());
                 CK(cudaEventRecord(e2, st));
                 launches += 2;

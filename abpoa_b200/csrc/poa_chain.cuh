@@ -23,6 +23,7 @@
 #ifndef POA_CHAIN_CUH
 #define POA_CHAIN_CUH
 
+#include <math.h>
 #include <stdint.h>
 #include "poa_device.cuh"
 
@@ -121,13 +122,15 @@ typedef struct PoaChainSlot {           /* one per read group; every pointer aim
  * caller's allocator `take(bytes)`, which also decides the alignment.  The engine carves a wave's HBM with it, its
  * wave planner sums the same requests, and the CPU emulator lays out its host buffer with it, so the three cannot
  * disagree.  The reads (chain_slot_reads) live in a region of their own: they are staged and uploaded in one copy.
- * `strand` (-s runs) adds the strand bytes and the second CIGAR buffer and result behind everything else. */
+ * `strand` (-s runs) adds the strand bytes and the second CIGAR buffer and result behind everything else.  `ps` (-G runs)
+ * makes the job blob room for the predscore section, one int per in-edge like pred. */
 template <class Take>
 static inline void chain_slot_layout(PoaChainSlot *s, int n_cap, int qmax, int n_reads, int K, int A, int m, int W, bool record, Take take,
-                                     bool strand = false) {
+                                     bool strand = false, bool ps = false) {
     const size_t nc = (size_t)n_cap, scr_n = nc > (size_t)qmax + 2 ? nc : (size_t)qmax + 2;
     s->n_cap = n_cap; s->pred_cap = (int32_t)(nc * 3); s->n_reads = n_reads;
     s->blob_cap = (int32_t)(256 + (nc + 1) * 8 + (size_t)s->pred_cap * 4 + 4 + (size_t)qmax + 64);
+    if (ps) s->blob_cap += (int32_t)((size_t)s->pred_cap * 4 + 4 + 16);
     s->jd.cigar_cap = (int32_t)(qmax + n_cap + 8);
     s->base = (uint8_t *)take(nc);
     s->in_cnt = (int32_t *)take(nc * 4); s->out_cnt = (int32_t *)take(nc * 4); s->aln_cnt = (int32_t *)take(nc * 4); s->n_read = (int32_t *)take(nc * 4);
@@ -288,6 +291,18 @@ POA_DEV bool chain_weak_hit(int best_score, int qlen, int node_n, int max_mat) {
     return best_score < lim * max_mat * .3333;
 }
 
+/* -G: the score of an in-edge of weight edge_w whose tail's out-edges weigh node_w in all, max(round(ln(edge_w / node_w)), -20),
+ * 0 if either weight is 0 (reference src/abpoa_graph.c:429-437; host twin poa_edge_path_score in poa_graph.c).  The device's
+ * log may differ from glibc's in the last bit; the chain admits node weights up to POA_PS_MAX_NODE_W only, and for those no
+ * ratio lies within 1024 ulp of a rounding boundary -(k + 1/2) (tests/test_chain_emul_ps.py proves it), so both round
+ * alike. */
+#define POA_PS_MAX_NODE_W (1 << 20)
+POA_DEV int chain_path_score(int edge_w, int node_w) {
+    if (node_w == 0 || edge_w == 0) return 0;
+    const int s = (int)round(log((double)edge_w / (double)node_w));
+    return s > -20 ? s : -20;
+}
+
 /* complement of a base code (reference src/abpoa_align.c:329): 0..3 -> 3..0, everything else -> 4, with -c too */
 POA_DEV uint8_t chain_comp(uint8_t b) { return b < 4 ? (uint8_t)(3 - b) : (uint8_t)4; }
 
@@ -346,7 +361,9 @@ POA_DEV void chain_set_remain(PoaChainSlot *s, int K, const int32_t *order, int 
 
 /* Flatten the graph + read `r` into the slot's job blob (layout: PoaJobHeader; the host twin is
  * poa_blob_fill in poa_flat.c).  Also the last line of defence for the order: every predecessor row
- * must be smaller than its row. */
+ * must be smaller than its row.  PS (-G runs; the host picks the fuse kernels' instantiation, so a run without -G compiles
+ * to the bare flatten): the predscore section behind pred, every in-edge's chain_path_score. */
+template <bool PS = false>
 POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int32_t *order, int n, int r, int pool_parity, int generous) {
     const int K = cp->K;
     int32_t *cnt = s->scr[0];
@@ -360,6 +377,7 @@ POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int3
     size_t off = chain_al16(sizeof(PoaJobHeader));
     const size_t off_rowmeta = off; off += chain_al16(((size_t)n + 1) * 8);
     const size_t off_pred = off; off += chain_al16((size_t)n_pred * 4 + 4);
+    const size_t off_ps = off; if (PS) off += chain_al16((size_t)n_pred * 4 + 4);
     const size_t off_qs = off; off += chain_al16((size_t)qlen + 1) + 16;
     if (off > (size_t)s->blob_cap || n_pred > s->pred_cap) {
         if (POA_TID0) { POA_ATOMIC_OR(&s->failed, POA_CF_BLOB_CAP); h->n_rows = 0; }
@@ -367,6 +385,7 @@ POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int3
         return;
     }
     int32_t *rowmeta = reinterpret_cast<int32_t *>(blob + off_rowmeta), *pred = reinterpret_cast<int32_t *>(blob + off_pred);
+    int32_t *pscore = reinterpret_cast<int32_t *>(blob + off_ps);
     uint8_t *qs = blob + off_qs;
     POA_PAR_FOR(i, n) {
         const int v = order[i];
@@ -380,6 +399,13 @@ POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int3
                 const int pr = s->node_row[iid[e]];
                 if (pr >= i) POA_ATOMIC_OR(&s->failed, POA_CF_ORDER);
                 pred[po + e] = pr;
+                if (PS) {                                       /* the in-edge's weight over its tail's out-edge weights */
+                    const int u = iid[e], no = s->out_cnt[u];
+                    const int32_t *ow = s->out_w + (size_t)u * K;
+                    int node_w = 0;
+                    for (int o = 0; o < no; ++o) node_w += ow[o];
+                    pscore[po + e] = chain_path_score(s->in_w[(size_t)v * K + e], node_w);
+                }
             }
         }
     }
@@ -389,7 +415,7 @@ POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int3
     if (POA_TID0) {
         rowmeta[2 * n] = n_pred; rowmeta[2 * n + 1] = 0;
         h->qlen = qlen; h->w = s->read_w[r]; h->node_n = n;
-        h->off_rowmeta = (int32_t)off_rowmeta; h->off_pred = (int32_t)off_pred; h->off_predscore = -1; h->off_live = -1;
+        h->off_rowmeta = (int32_t)off_rowmeta; h->off_pred = (int32_t)off_pred; h->off_predscore = PS ? (int32_t)off_ps : -1; h->off_live = -1;
         h->off_qs = (int32_t)off_qs; h->rsv[0] = h->rsv[1] = h->rsv[2] = h->rsv[3] = 0;
         h->blob_bytes = (int32_t)off; h->pn = chain_ref_pn(cp, qlen, n); h->pad[0] = h->pad[1] = 0;
 #ifndef POA_CHAIN_EMUL
@@ -420,7 +446,8 @@ POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int3
 
 /* ------------------------------------------------------------------ first read of a group */
 /* a chain SRC -> b0 -> b1 ... -> SINK (reference src/abpoa_graph.c:573-593): the edge into b_i weighs w[i], the edge into
- * SINK w[len - 1] */
+ * SINK w[len - 1]; PS: see chain_flatten */
+template <bool PS = false>
 POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
     const int K = cp->K;
     ChainRead rd = chain_read(s, 0);
@@ -457,7 +484,7 @@ POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
     if (POA_TID0) { s->n_nodes = n; s->cur = 0; s->fused = 1; s->retry = 0; if (s->read_rc) s->read_rc[0] = 0; }   /* read 0 seeds: no strand test */
     POA_CTA_SYNC();
     chain_set_remain(s, K, order, n);
-    if (s->n_reads > 1) chain_flatten(s, cp, order, n, 1, /*pool_parity=*/1, 0);
+    if (s->n_reads > 1) chain_flatten<PS>(s, cp, order, n, 1, /*pool_parity=*/1, 0);
 }
 
 /* ------------------------------------------------------------------ fuse read r, prepare read r + 1 */
@@ -467,7 +494,9 @@ POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
 #define CK_NEWI 2       /* inserted base: new unaligned node                                                  */
 
 /* `round`: the round of the cohort's schedule that just ran (the next alignment kernel is round + 1; its plane pool is
- * the one with that parity).  A group normally fuses read `round`, but one that had to re-run an alignment lags behind. */
+ * the one with that parity).  A group normally fuses read `round`, but one that had to re-run an alignment lags behind.
+ * PS: see chain_flatten. */
+template <bool PS = false>
 POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
     const int K = cp->K, A = cp->A;
     const int r = s->fused;                                /* the read whose alignment just finished */
@@ -478,7 +507,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
     if (res->status == POA_ST_PLANE_OVF && !s->retry && s->pool_cursor) {   /* band wider than the slab: same read again, full-rectangle slab */
         POA_CTA_SYNC();
         if (POA_TID0) s->retry = 1;
-        chain_flatten(s, cp, s->order[s->cur], s->n_nodes, r, round + 1, 1);
+        chain_flatten<PS>(s, cp, s->order[s->cur], s->n_nodes, r, round + 1, 1);
         return;
     }
     if (res->status != POA_ST_OK) {
@@ -678,7 +707,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
 
     /* ---- 9. band centres and the next job ---- */
     chain_set_remain(s, K, order_new, n);
-    if (r + 1 < s->n_reads) chain_flatten(s, cp, order_new, n, r + 1, round + 1, 0);
+    if (r + 1 < s->n_reads) chain_flatten<PS>(s, cp, order_new, n, r + 1, round + 1, 0);
     else if (POA_TID0) hdr->n_rows = 0;
     POA_CTA_SYNC();
 }

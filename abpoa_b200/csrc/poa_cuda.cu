@@ -135,6 +135,7 @@ struct poa_dev_ctx {
     poa_pressure_fn pressure; void *pressure_user;   /* called before this context WAITS for plane memory */
     PoaJobDesc last_desc; int last_bits, last_gap, last_rows;   /* debug: job 0 of the most recent launch */
     int last_lean, last_tma, last_ring_rows, last_ring_cells; uint64_t last_units;   /* ... how it ran, and its plane units used */
+    int last_ps;                        /* ... a whole-graph global -G run of the packed kernel (LEAN but for its path scores) */
 };
 
 static void require_gpu(void) {
@@ -152,7 +153,7 @@ poa_dev_ctx *poa_dev_ctx_new_on(int dev) {
     c->h_in_cap = c->h_out_cap = c->d_in_cap = c->d_work_cap = c->d_planes_cap = c->h_res_cap = c->planes_limit = 0;
     memset(&c->stats, 0, sizeof c->stats); c->capture = NULL; c->capture_user = NULL; c->pressure = NULL; c->pressure_user = NULL; memset(&c->last_desc, 0, sizeof c->last_desc);
     c->last_bits = c->last_gap = c->last_rows = 0;
-    c->last_lean = c->last_tma = c->last_ring_rows = c->last_ring_cells = 0; c->last_units = 0;
+    c->last_lean = c->last_tma = c->last_ring_rows = c->last_ring_cells = 0; c->last_units = 0; c->last_ps = 0;
     if (dev >= 0) { c->dev = dev; CK(cudaSetDevice(c->dev)); }
     else CK(cudaGetDevice(&c->dev));
     CK(cudaStreamCreateWithFlags(&c->st, cudaStreamNonBlocking));
@@ -363,8 +364,10 @@ static bool run_begin(poa_dev_ctx *c, const abpoa_para_t *abpt, poa_job *jobs, c
     static const size_t smem_budget = [] { const char *e = getenv("ABPOA_GPU_SMEM_KB"); return (size_t)(e && *e ? atoi(e) : 28) * 1024; }();
     int ring_rows = 2, ring_cells = 64;
     poa_pick_ring(abpt->gap_mode, bits == 32 ? 32 : 16, band_cells, smem_budget, &ring_rows, &ring_cells);
-    int lean = !abpt->inc_path_score && abpt->align_mode == ABPOA_GLOBAL_MODE;
-    for (int t = 0; t < n && lean; ++t) if (!jobs[idx[t]].plan.whole_graph) lean = 0;
+    int whole = abpt->align_mode == ABPOA_GLOBAL_MODE;
+    for (int t = 0; t < n && whole; ++t) if (!jobs[idx[t]].plan.whole_graph) whole = 0;
+    int lean = whole && !abpt->inc_path_score;
+    c->last_ps = bits == 15 && whole && abpt->inc_path_score && !poa_lean_disabled();
     const int gaps[4] = { abpt->gap_ext1, abpt->gap_open1 + abpt->gap_ext1, abpt->gap_ext2, abpt->gap_open2 + abpt->gap_ext2 };
     /* what poa_launch_align_p16 will instantiate (the TMA variant exists only with LEAN) */
     c->last_lean = bits == 15 && lean && !poa_lean_disabled(); c->last_tma = c->last_lean && poa_tma_enabled();
@@ -703,23 +706,25 @@ extern "C" int poa_debug_last_run(abpoa_t *ab, int32_t *out8) {
  * row's slab offset: cap / 2 bytes), the graph-CIGAR (node ids, in abpoa_res_t order) and out[16] = status, best score,
  * node_e, query_e, node_s, query_s, n_ops, cells, max_band, plane_units_used, ring_rows, ring_cells, buf_cells,
  * windows recomputed (all rows), windows of the row with the most.
- * Returns -1 unless the last accepted run was the packed LEAN global kernel with affine or convex gaps, -2 for a ring that
+ * A -G alignment (its blob has path scores: off_predscore >= 0) that would have run LEAN but for its path scores replays on
+ * the job function's path-score instantiation, as the chain runs -G jobs.
+ * Returns -1 unless the last accepted run was the packed LEAN global kernel (or such a -G run) with affine or convex gaps, -2 for a ring that
  * does not fit one CTA or a buffer that does not fit shared memory; else the slab capacity the outputs need (bytes) when
  * `slab` is NULL or `cap` is smaller, else the bytes of the compact slab the replay used.  Nothing of the chain's or the
  * launch engine's own path runs here. */
 extern "C" cudaError_t poa_launch_chain_replay(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int ring_rows, int ring_cells,
-                                               cudaStream_t st);
+                                               int ps, cudaStream_t st);
 extern "C" cudaError_t poa_launch_fb_dump(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int n_rows, int buf_cells,
-                                          int16_t *fslab, uint8_t *fbits, int32_t *windows, cudaStream_t st);
+                                          int16_t *fslab, uint8_t *fbits, int32_t *windows, int ps, cudaStream_t st);
 extern "C" int poa_chain_fb_buf_cells(int gap_mode, int ring_rows, int ring_cells);
 extern "C" int64_t poa_debug_chain_replay(abpoa_t *ab, int ring_rows, int ring_cells, int buf_cells, int32_t *rowinfo, uint32_t *rowoff,
                                           void *slab, void *fslab, uint8_t *fbits, int64_t cap, uint64_t *cigar, int64_t cigar_cap, int64_t *out16) {
     poa_dev_ctx *c = (poa_dev_ctx *)ab->abm->s_mem;
-    if (!c || c->arena || c->last_rows <= 0 || c->last_bits != 15 || !c->last_lean) return -1;
+    if (!c || c->arena || c->last_rows <= 0 || c->last_bits != 15 || !(c->last_lean || c->last_ps)) return -1;
     if (c->last_gap != ABPOA_AFFINE_GAP && c->last_gap != ABPOA_CONVEX_GAP) return -1;
     CK(cudaSetDevice(c->dev));
     PoaJobHeader hd; CK(cudaMemcpy(&hd, c->last_desc.blob, sizeof hd, cudaMemcpyDeviceToHost));
-    const int n_rows = hd.n_rows, qlen = hd.qlen, gap = c->last_gap;
+    const int n_rows = hd.n_rows, qlen = hd.qlen, gap = c->last_gap, ps = hd.off_predscore >= 0;
     const int n16 = gap == ABPOA_AFFINE_GAP ? 2 : 3;
     const uint64_t units = (uint64_t)((qlen + 1 + 7) / 8 + 1) * n16 * n_rows;      /* full rectangle: no PLANE_OVF */
     const int64_t need = (int64_t)units * POA_GROUP * 2;
@@ -743,7 +748,7 @@ extern "C" int64_t poa_debug_chain_replay(abpoa_t *ab, int ring_rows, int ring_c
     jd.result = (PoaResultDev *)d; jd.rowinfo = (PoaRowInfo *)(d + o_ri); jd.rowoff = (PoaRowOff *)(d + o_ro);
     jd.cigar = (uint64_t *)(d + o_cg); jd.cigar_cap = (int32_t)cg_cap; jd.btrec = (PoaBtRec *)(d + o_bt);
     jd.planes = d + o_sl; jd.plane_cap_units = units;
-    const cudaError_t le = poa_launch_chain_replay(gap, gaps, &jd, (const PoaParamsDev *)c->d_in, ring_rows, ring_cells, c->st);
+    const cudaError_t le = poa_launch_chain_replay(gap, gaps, &jd, (const PoaParamsDev *)c->d_in, ring_rows, ring_cells, ps, c->st);
     if (le == cudaErrorInvalidValue) { cudaGetLastError(); CK(cudaFree(d)); return -2; }
     CK(le);
     PoaResultDev r; CK(cudaMemcpyAsync(&r, d, sizeof r, cudaMemcpyDeviceToHost, c->st));
@@ -758,7 +763,7 @@ extern "C" int64_t poa_debug_chain_replay(abpoa_t *ab, int ring_rows, int ring_c
     std::vector<int32_t> win(n_rows, 0);
     if (r.status == POA_ST_OK) {                        /* every row record is written: the dump reads inside the slab only */
         const cudaError_t de = poa_launch_fb_dump(gap, gaps, &jd, (const PoaParamsDev *)c->d_in, n_rows, buf_cells, (int16_t *)(d + o_fs), d + o_fb,
-                                                  (int32_t *)(d + o_wn), c->st);
+                                                  (int32_t *)(d + o_wn), ps, c->st);
         if (de == cudaErrorInvalidValue) { cudaGetLastError(); CK(cudaFree(d)); return -2; }
         CK(de);
         CK(cudaMemcpyAsync(fslab, d + o_fs, (size_t)need, cudaMemcpyDeviceToHost, c->st));

@@ -197,11 +197,11 @@ struct FbCtx {
 /* fb_recompute<..., DUMP = true> (debug export poa_debug_chain_replay only): also stores the recomputed F1 (/ F2) of the
  * kept passes, F1 of group g at f + 8 (g - g0), F2 fstride cells later -- the row's F planes as the five-plane layout holds them */
 struct FbDumpCtx : FbCtx { int16_t *f; int fstride; };
-template <int GAP, int MODE, bool DUMP = false>
+template <int GAP, int MODE, bool DUMP = false, bool PS = false>
 __device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaParamsDev *prm, const FbCtx &fx,
                             int beg, int end, int pb, int np, int base, int j, int lane);
 
-template <int GAP, typename ST, int MODE, bool FB = false>
+template <int GAP, typename ST, int MODE, bool FB = false, bool PS = false>
 __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const PoaParamsDev *prm, const int *mat_s,
                               int lane, int best_i, int best_j, PoaResultDev &res, int xs = 3, const PoaBtRec *btrec = nullptr,
                               const FbCtx *fx = nullptr) {
@@ -486,7 +486,7 @@ __device__ void poa_backtrack(const JobView &jv, const PoaJobDesc &jd, const Poa
                 if (h_jm1 - e1 == h_ij) hit = 1;
             } else if constexpr (RL::BITS) {                            /* the comparisons below, on the recomputed F planes */
                 if (in_j && (i != fb_row || j < fb_lo)) {               /* first insertion step of this row (or left of the window) */
-                    fb_lo = fb_recompute<GAP, MODE>(jv, jd, prm, *fx, me.beg, me.end, me.pb, me.np, me.base, j, lane);
+                    fb_lo = fb_recompute<GAP, MODE, false, PS>(jv, jd, prm, *fx, me.beg, me.end, me.pb, me.np, me.base, j, lane);
                     fb_row = i;
 #ifdef POA_KPROF
                     ++bd_fbrows;
@@ -1160,8 +1160,9 @@ __device__ __forceinline__ uint2 p16_fbits(const P16Consts &kc, const unsigned H
 /* Recompute row `row`'s F planes for the backtrace's insertion step (compact layout): the row arithmetic of the forward pass
  * (p16_cells), fed from the predecessors' H / E planes in HBM, the query profile and the band-mask tables, pass by pass from
  * the band's first cell to cell j.  The decision bytes of the last fx.buf_cells / 256 passes up to j's go to fx.buf, from the
- * returned cell on.  Jobs of the compact layout run the LEAN forward pass, which has no path scores (chain jobs carry none). */
-template <int GAP, int MODE, bool DUMP>
+ * returned cell on.  PS (-G jobs of the chain): predecessor k's path score is added to its diagonal term and its E planes,
+ * as the forward pass adds it, so the recomputed planes match the forward pass bit for bit. */
+template <int GAP, int MODE, bool DUMP, bool PS>
 __device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaParamsDev *prm, const FbCtx &fx,
                             int beg, int end, int pb, int np, int base, int j, int lane) {
     const P16Consts &kc = *fx.kc;
@@ -1186,11 +1187,12 @@ __device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaPa
         for (int k = 0; k < 4; ++k) { M[k] = NEGP2; X1[k] = NEGP2; X2[k] = NEGP2; }
         const bool fix_left = (gp > g0) || ((beg & 7) == 0);
         for (int kb = 0; kb < np; kb += 32) {
-            int c_g0 = 0, c_ng = 0; uint32_t c_off = 0;                /* predecessor kb + lane: first group, groups, slab offset */
+            int c_g0 = 0, c_ng = 0, c_ps = 0; uint32_t c_off = 0;      /* predecessor kb + lane: first group, groups, path score, slab offset */
             if (kb + lane < np) {
                 const int prow = ldb(jv.pred + pb + kb + lane);
                 const PoaRowInfo pi = jd.rowinfo[prow];
                 c_g0 = pi.beg >> 3; c_ng = (pi.end >> 3) - c_g0 + 1; c_off = jd.rowoff[prow].off;
+                if (PS) c_ps = ldb(jv.predscore + pb + kb + lane);
             }
             const int nk = min(32, np - kb);
             for (int k = 0; k < nk; ++k) {
@@ -1213,8 +1215,20 @@ __device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaPa
                     if (MODE == LOCAL && g == 0) hm1 = 0;
                     prev = (unsigned)hm1 << 16;
                 }
-                M[0] = __vmaxs2(M[0], sh1(prev, hp.x)); M[1] = __vmaxs2(M[1], sh1(hp.x, hp.y));
-                M[2] = __vmaxs2(M[2], sh1(hp.y, hp.z)); M[3] = __vmaxs2(M[3], sh1(hp.z, hp.w));
+                unsigned d0 = sh1(prev, hp.x), d1 = sh1(hp.x, hp.y), d2 = sh1(hp.y, hp.z), d3 = sh1(hp.z, hp.w);
+                if (PS) {
+                    const int ps = __shfl_sync(FULL, c_ps, k);
+                    const unsigned ps2 = pk(ps, ps);
+                    d0 = __viaddmax_s16x2(d0, ps2, NEGP2); d1 = __viaddmax_s16x2(d1, ps2, NEGP2);
+                    d2 = __viaddmax_s16x2(d2, ps2, NEGP2); d3 = __viaddmax_s16x2(d3, ps2, NEGP2);
+                    ep1.x = __viaddmax_s16x2(ep1.x, ps2, NEGP2); ep1.y = __viaddmax_s16x2(ep1.y, ps2, NEGP2);
+                    ep1.z = __viaddmax_s16x2(ep1.z, ps2, NEGP2); ep1.w = __viaddmax_s16x2(ep1.w, ps2, NEGP2);
+                    if (GAP == CG) {
+                        ep2.x = __viaddmax_s16x2(ep2.x, ps2, NEGP2); ep2.y = __viaddmax_s16x2(ep2.y, ps2, NEGP2);
+                        ep2.z = __viaddmax_s16x2(ep2.z, ps2, NEGP2); ep2.w = __viaddmax_s16x2(ep2.w, ps2, NEGP2);
+                    }
+                }
+                M[0] = __vmaxs2(M[0], d0); M[1] = __vmaxs2(M[1], d1); M[2] = __vmaxs2(M[2], d2); M[3] = __vmaxs2(M[3], d3);
                 X1[0] = __vmaxs2(X1[0], ep1.x); X1[1] = __vmaxs2(X1[1], ep1.y); X1[2] = __vmaxs2(X1[2], ep1.z); X1[3] = __vmaxs2(X1[3], ep1.w);
                 if (GAP == CG) { X2[0] = __vmaxs2(X2[0], ep2.x); X2[1] = __vmaxs2(X2[1], ep2.y); X2[2] = __vmaxs2(X2[2], ep2.z); X2[3] = __vmaxs2(X2[3], ep2.w); }
             }
@@ -1252,7 +1266,10 @@ __device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaPa
  * stores per lane; a slot is reused ring_rows rows later, after cp.async.bulk.wait_group.read says the engine has
  * finished reading it.  Rows wider than a ring slot keep the plain stores. */
 /* FB: the compact row layout (RowLayout): no F planes; the backtrace recomputes them where it needs them (fb_recompute). */
-template <int GAP, int MODE, bool LEAN = false, bool TMA = false, bool FB = false>
+/* PS (with LEAN; the chain's -G jobs): the job carries path scores.  The straight-line rows add predecessor k's score to its
+ * diagonal term and its E planes (linear gaps: to H before - e1), the arithmetic of the general rows, with the scores of the
+ * row's first LP predecessors broadcast one row ahead next to their rows.  Without PS a LEAN job carries none. */
+template <int GAP, int MODE, bool LEAN = false, bool TMA = false, bool FB = false, bool PS = false>
 __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParamsDev *__restrict__ prm, const P16Consts &kc, const P16Smem &sm,
                                             int ring_rows, int ring_cells, int lane) {
     static_assert(!(TMA && FB), "the TMA row drain stages the five-plane layout");
@@ -1348,7 +1365,7 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
     const int pn_shift = pnv == 16 ? 4 : 3;
     const uint32_t cap32 = jd.plane_cap_units > 0xffffffffull ? 0xffffffffu : (uint32_t)jd.plane_cap_units;
     uint32_t cur32 = (uint32_t)cursor;
-    const bool has_ps = LEAN ? false : (jv.predscore != nullptr);
+    const bool has_ps = LEAN ? PS : (jv.predscore != nullptr);
 
     /* Graph metadata runs one full row ahead of its use: what iteration i loads (row i+1's list end, residue / band centre
      * and -- unconditionally, clamped to the list -- its per-lane predecessor entries) is first touched at the top of
@@ -1362,17 +1379,20 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
     }
     int nx_y = n_rows > 3 ? ldb(&jv.rowmeta[2].y) : 0;          /* packed (remain, residue) of row i+1 */
     constexpr int LP = 4;                                     /* LEAN: up to LP predecessors per row on the straight-line path (> 2: 14 % of the rows at 10 kbp x 50) */
-    int lp_c[LP];                                             /* the coming row's first LP predecessors, broadcast off the row-to-row chain */
+    int lp_c[LP], lps_c[LP];                                  /* the coming row's first LP predecessors (and -G scores), broadcast off the row-to-row chain */
 #pragma unroll
-    for (int k = 0; k < LP; ++k) lp_c[k] = LEAN ? __shfl_sync(FULL, lane < pe - pb ? raw_pred : -1, k) : -1;
+    for (int k = 0; k < LP; ++k) {
+        lp_c[k] = LEAN ? __shfl_sync(FULL, lane < pe - pb ? raw_pred : -1, k) : -1;
+        lps_c[k] = PS ? __shfl_sync(FULL, lane < pe - pb ? raw_ps : 0, k) : 0;
+    }
     KP_DECL
     for (int i = 1; i < n_rows - 1 && !stop; ++i) {
         KP(5)
         const int np = pe - pb;
         const int mypred = lane < np ? raw_pred : -1, myps = lane < np ? raw_ps : 0;
-        int lp[LP];                                           /* the row's first LP predecessors, known to every lane (broadcast at the end of the previous iteration) */
+        int lp[LP], lps[LP];                                  /* the row's first LP predecessors and scores, known to every lane (broadcast at the end of the previous iteration) */
 #pragma unroll
-        for (int k = 0; k < LP; ++k) lp[k] = lp_c[k];
+        for (int k = 0; k < LP; ++k) { lp[k] = lp_c[k]; lps[k] = lps_c[k]; }
         /* unconditional: rowmeta has n_rows + 1 entries and i + 2 <= n_rows; the predecessor index is clamped (a predicated
          * load would need a select on its result, which the compiler schedules right behind the load) */
         int2 m2;                                              /* two 32-bit loads: a 64-bit one ties up an aligned register pair that ptxas frees by
@@ -1517,7 +1537,23 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
                             prev = (unsigned)hm1 << 16;
                         }
                     } else if (lane == 0) prev = (MODE == LOCAL && g == 0) ? 0u : ((unsigned)NEGP << 16);
-                    const unsigned d0 = sh1(prev, hp.x), d1 = sh1(hp.x, hp.y), d2 = sh1(hp.y, hp.z), d3 = sh1(hp.z, hp.w);
+                    unsigned d0 = sh1(prev, hp.x), d1 = sh1(hp.x, hp.y), d2 = sh1(hp.y, hp.z), d3 = sh1(hp.z, hp.w);
+                    if (PS) {
+                        const unsigned ps2 = pk(lps[k], lps[k]);
+                        d0 = __viaddmax_s16x2(d0, ps2, NEGP2); d1 = __viaddmax_s16x2(d1, ps2, NEGP2);
+                        d2 = __viaddmax_s16x2(d2, ps2, NEGP2); d3 = __viaddmax_s16x2(d3, ps2, NEGP2);
+                        if (GAP == LG) {
+                            hp.x = __viaddmax_s16x2(hp.x, ps2, NEGP2); hp.y = __viaddmax_s16x2(hp.y, ps2, NEGP2);
+                            hp.z = __viaddmax_s16x2(hp.z, ps2, NEGP2); hp.w = __viaddmax_s16x2(hp.w, ps2, NEGP2);
+                        } else {
+                            ep1.x = __viaddmax_s16x2(ep1.x, ps2, NEGP2); ep1.y = __viaddmax_s16x2(ep1.y, ps2, NEGP2);
+                            ep1.z = __viaddmax_s16x2(ep1.z, ps2, NEGP2); ep1.w = __viaddmax_s16x2(ep1.w, ps2, NEGP2);
+                            if (GAP == CG) {
+                                ep2.x = __viaddmax_s16x2(ep2.x, ps2, NEGP2); ep2.y = __viaddmax_s16x2(ep2.y, ps2, NEGP2);
+                                ep2.z = __viaddmax_s16x2(ep2.z, ps2, NEGP2); ep2.w = __viaddmax_s16x2(ep2.w, ps2, NEGP2);
+                            }
+                        }
+                    }
                     if (GAP == LG) {
                         hp.x = __viaddmax_s16x2(hp.x, kc.NE1, NEGP2); hp.y = __viaddmax_s16x2(hp.y, kc.NE1, NEGP2); hp.z = __viaddmax_s16x2(hp.z, kc.NE1, NEGP2); hp.w = __viaddmax_s16x2(hp.w, kc.NE1, NEGP2);
                     }
@@ -1727,7 +1763,10 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
         asm volatile("" : "+r"(m2.x), "+r"(m2.y), "+r"(n_raw_pred), "+r"(n_raw_ps));
         pb = pe; pe = m2.x; rbase = n_rbase; rem = n_rem; nx_y = m2.y; raw_pred = n_raw_pred; raw_ps = n_raw_ps;
 #pragma unroll
-        for (int k = 0; k < LP; ++k) lp_c[k] = LEAN ? __shfl_sync(FULL, lane < pe - pb ? raw_pred : -1, k) : -1;
+        for (int k = 0; k < LP; ++k) {
+            lp_c[k] = LEAN ? __shfl_sync(FULL, lane < pe - pb ? raw_pred : -1, k) : -1;
+            lps_c[k] = PS ? __shfl_sync(FULL, lane < pe - pb ? raw_ps : 0, k) : 0;
+        }
     }
     cursor = cur32;
     KP_OUT(res)
@@ -1766,7 +1805,7 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
         FbCtx fx;                                            /* FB: the ring is free now and holds the recomputed decision bytes */
         fx.kc = &kc; fx.cap_lo = cap_lo; fx.cap_hi = cap_hi;
         fx.buf = reinterpret_cast<uint8_t *>(ring_data); fx.buf_cells = (int)ring_row_bytes * ring_rows;
-        poa_backtrack<GAP, ST, MODE, FB>(jv, jd, prm, mat_s, lane, best_i, best_j, *jd.result, 3, jd.btrec, &fx);
+        poa_backtrack<GAP, ST, MODE, FB, PS>(jv, jd, prm, mat_s, lane, best_i, best_j, *jd.result, 3, jd.btrec, &fx);
         if (lane == 0) jd.result->bt_clk = clock64() - clk1;
     }
 }
@@ -1803,15 +1842,15 @@ static inline size_t ring_smem_bytes(int gap, int bits, int ring_rows, int ring_
  * strictly more; its CIGAR words and result are then copied over the primary ones, so the fuse reads one place either
  * way.  The primary result carries the DP cells and cycles of both passes and the first status that is not OK (a failed
  * pair is re-run or handed back like a failed alignment); read_rc[r] records the strand (bit 0) and whether the retry
- * ran (bit 1). */
-template <int GAP, bool STRAND>
+ * ran (bit 1).  PS (-G; the host picks the instantiation): the job blob carries path scores (p16_run_job). */
+template <int GAP, bool STRAND, bool PS>
 __device__ __forceinline__ void chain_align_read(const PoaJobDesc &jd, const PoaChainSlot *sl, const PoaChainParams *__restrict__ cp,
                                                  const PoaParamsDev *__restrict__ prm, const P16Consts &kc, const P16Smem &sm, int ring_rows, int ring_cells,
                                                  int lane) {
     PoaJobDesc jp = jd;
     bool second = false;
     for (int pass = 0; pass < (STRAND ? 2 : 1); ++pass) {
-        p16_run_job<GAP, GLOBAL, true, false, true>(jp, prm, kc, sm, ring_rows, ring_cells, lane);
+        p16_run_job<GAP, GLOBAL, true, false, true, PS>(jp, prm, kc, sm, ring_rows, ring_cells, lane);
         __syncwarp();
         if (!STRAND || pass) break;
         const PoaJobHeader *h = reinterpret_cast<const PoaJobHeader *>(jd.blob);
@@ -1846,7 +1885,7 @@ __device__ __forceinline__ void chain_align_read(const PoaJobDesc &jd, const Poa
  * The same job function, fed from device-resident slots (poa_chain.cuh): the job blob of a slot is written
  * by the fuse kernel of the previous round, nothing comes from the host.  Block 0 also zeroes the plane-pool
  * cursor the coming fuse kernel will fill (see PoaChainSlot). */
-template <int GAP, bool STRAND>
+template <int GAP, bool STRAND, bool PS>
 __global__ void POA_P16_BOUNDS poa_chain_align_kernel_p16(const PoaChainSlot *__restrict__ slots, const int32_t *__restrict__ idx,
                                                            const PoaChainParams *__restrict__ cp, const PoaParamsDev *__restrict__ prm, int n_jobs,
                                                            int round, int ring_rows, int ring_cells, const __grid_constant__ P16Consts kc) {
@@ -1860,7 +1899,7 @@ __global__ void POA_P16_BOUNDS poa_chain_align_kernel_p16(const PoaChainSlot *__
     const int n_rows = reinterpret_cast<const PoaJobHeader *>(jd.blob)->n_rows;
     if (sl->failed || sl->fused >= sl->n_reads || n_rows < 3) { if (lane == 0) jd.result->status = POA_ST_SKIP; return; }
     const P16Smem sm = p16_smem_init(dyn_smem, prm, ring_rows, lane);
-    chain_align_read<GAP, STRAND>(jd, sl, cp, prm, kc, sm, ring_rows, ring_cells, lane);
+    chain_align_read<GAP, STRAND, PS>(jd, sl, cp, prm, kc, sm, ring_rows, ring_cells, lane);
 }
 
 /* Free-running chain (PoaChainSync in poa_chain.cuh): one resident warp per group runs the group's alignments back to
@@ -1870,7 +1909,7 @@ __device__ __forceinline__ int chain_ld_relaxed(const int32_t *p) { int v; asm v
 __device__ __forceinline__ void chain_st_relaxed(int32_t *p, int v) { asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ unsigned long long chain_now_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
-template <int GAP, bool STRAND>
+template <int GAP, bool STRAND, bool PS>
 __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, PoaChainSync *sync, const PoaChainParams *__restrict__ cp,
                                                           const PoaParamsDev *__restrict__ prm, int n_groups, int ring_rows, int ring_cells, int dbg,
                                                           const __grid_constant__ P16Consts kc) {
@@ -1910,7 +1949,7 @@ __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, P
         const PoaJobDesc jd = sl->jd;
         const int n_rows = reinterpret_cast<const PoaJobHeader *>(jd.blob)->n_rows;
         if (sl->failed || sl->fused >= sl->n_reads || n_rows < 3) break;
-        chain_align_read<GAP, STRAND>(jd, sl, cp, prm, kc, sm, ring_rows, ring_cells, lane);
+        chain_align_read<GAP, STRAND, PS>(jd, sl, cp, prm, kc, sm, ring_rows, ring_cells, lane);
         __syncwarp();
         if (!(dbg & 1)) __threadfence();                       /* release side: CIGAR + result are out before the task is */
         if (lane == 0) {
@@ -1929,7 +1968,7 @@ __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, P
     }
 }
 
-template <int GAP, bool STRAND>
+template <int GAP, bool STRAND, bool PS>
 static cudaError_t launch_chain_worker_one(PoaChainSlot *slots, PoaChainSync *sync, int n_groups, const PoaChainParams *cp, const PoaParamsDev *prm,
                                            int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
     /* at least 23 KB: at most 9 of these CTAs fit one SM, which leaves registers (9 x 160 x 32 of 64 K) and shared memory for a
@@ -1938,53 +1977,60 @@ static cudaError_t launch_chain_worker_one(PoaChainSlot *slots, PoaChainSync *sy
     static const int dbg = [] { const char *e = getenv("ABPOA_GPU_CHAIN_DBG"); return e && *e ? atoi(e) : 0; }();
     const size_t smem0 = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
     const size_t smem = (dbg & 2) ? smem0 : std::max<size_t>(smem0, (size_t)23 * 1024);
-    cudaError_t e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, STRAND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, STRAND, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return e;
     /* the same L1/shared split as the fuse workers ask for (poa_chain.cu): CTAs of both kernels share SMs for the whole run */
     { const char *cv = getenv("ABPOA_GPU_CHAIN_CARVEOUT");
-      e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, STRAND>, cudaFuncAttributePreferredSharedMemoryCarveout, cv && *cv ? atoi(cv) : (int)cudaSharedmemCarveoutMaxShared);
+      e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, STRAND, PS>, cudaFuncAttributePreferredSharedMemoryCarveout, cv && *cv ? atoi(cv) : (int)cudaSharedmemCarveoutMaxShared);
       if (e != cudaSuccess) return e; }
-    poa_chain_dp_worker_kernel<GAP, STRAND><<<n_groups, 32, smem, st>>>(slots, sync, cp, prm, n_groups, ring_rows, ring_cells, dbg, kc);
+    poa_chain_dp_worker_kernel<GAP, STRAND, PS><<<n_groups, 32, smem, st>>>(slots, sync, cp, prm, n_groups, ring_rows, ring_cells, dbg, kc);
     return cudaGetLastError();
 }
-/* strand: the host's PoaChainParams::amb_strand (-s), which picks the kernel instantiation */
+template <bool STRAND, bool PS>
+static cudaError_t launch_chain_worker_gap(int gap_mode, PoaChainSlot *slots, PoaChainSync *sync, int n_groups, const PoaChainParams *cp,
+                                           const PoaParamsDev *prm, int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
+    if (gap_mode == LG) return launch_chain_worker_one<LG, STRAND, PS>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == AG) return launch_chain_worker_one<AG, STRAND, PS>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    return launch_chain_worker_one<CG, STRAND, PS>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+}
+/* strand / ps: the host's PoaChainParams::amb_strand (-s) and whether the run has -G path scores, which pick the kernel instantiation */
 extern "C" cudaError_t poa_launch_chain_dp_worker(int gap_mode, const int *gaps, PoaChainSlot *slots, PoaChainSync *sync, int n_groups,
-                                                  const PoaChainParams *cp, int strand, const PoaParamsDev *prm, int ring_rows, int ring_cells, cudaStream_t st) {
+                                                  const PoaChainParams *cp, int strand, int ps, const PoaParamsDev *prm, int ring_rows, int ring_cells,
+                                                  cudaStream_t st) {
     if (n_groups <= 0) return cudaSuccess;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    if (strand) {
-        if (gap_mode == LG) return launch_chain_worker_one<LG, true>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
-        if (gap_mode == AG) return launch_chain_worker_one<AG, true>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
-        return launch_chain_worker_one<CG, true>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
-    }
-    if (gap_mode == LG) return launch_chain_worker_one<LG, false>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
-    if (gap_mode == AG) return launch_chain_worker_one<AG, false>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
-    return launch_chain_worker_one<CG, false>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    if (strand) return ps ? launch_chain_worker_gap<true, true>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st)
+                          : launch_chain_worker_gap<true, false>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    return ps ? launch_chain_worker_gap<false, true>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st)
+              : launch_chain_worker_gap<false, false>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
 }
 
-template <int GAP, bool STRAND>
+template <int GAP, bool STRAND, bool PS>
 static cudaError_t launch_chain_one(const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round, const PoaChainParams *cp, const PoaParamsDev *prm,
                                     int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
     const size_t smem = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
-    cudaError_t e = cudaFuncSetAttribute(poa_chain_align_kernel_p16<GAP, STRAND>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_align_kernel_p16<GAP, STRAND, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return e;
-    poa_chain_align_kernel_p16<GAP, STRAND><<<n_jobs, 32, smem, st>>>(slots, idx, cp, prm, n_jobs, round, ring_rows, ring_cells, kc);
+    poa_chain_align_kernel_p16<GAP, STRAND, PS><<<n_jobs, 32, smem, st>>>(slots, idx, cp, prm, n_jobs, round, ring_rows, ring_cells, kc);
     return cudaGetLastError();
+}
+template <bool STRAND, bool PS>
+static cudaError_t launch_chain_gap(int gap_mode, const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round, const PoaChainParams *cp,
+                                    const PoaParamsDev *prm, int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
+    if (gap_mode == LG) return launch_chain_one<LG, STRAND, PS>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == AG) return launch_chain_one<AG, STRAND, PS>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    return launch_chain_one<CG, STRAND, PS>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
 }
 /* gaps[4] = { e1, oe1, e2, oe2 } (host copy of what prm holds on the device) */
 extern "C" cudaError_t poa_launch_chain_align_p16(int gap_mode, const int *gaps, const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round,
-                                                  const PoaChainParams *cp, int strand, const PoaParamsDev *prm, int ring_rows, int ring_cells,
+                                                  const PoaChainParams *cp, int strand, int ps, const PoaParamsDev *prm, int ring_rows, int ring_cells,
                                                   cudaStream_t st) {
     if (n_jobs <= 0) return cudaSuccess;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    if (strand) {
-        if (gap_mode == LG) return launch_chain_one<LG, true>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
-        if (gap_mode == AG) return launch_chain_one<AG, true>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
-        return launch_chain_one<CG, true>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
-    }
-    if (gap_mode == LG) return launch_chain_one<LG, false>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
-    if (gap_mode == AG) return launch_chain_one<AG, false>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
-    return launch_chain_one<CG, false>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    if (strand) return ps ? launch_chain_gap<true, true>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st)
+                          : launch_chain_gap<true, false>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    return ps ? launch_chain_gap<false, true>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st)
+              : launch_chain_gap<false, false>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
 }
 
 /* ------------------------------------------------------------------ debug: the chain's job function on one job
@@ -1994,16 +2040,16 @@ extern "C" cudaError_t poa_launch_chain_align_p16(int gap_mode, const int *gaps,
  * the row's last cell first, then at the cell left of the previous window, down to the band's first cell.  It keeps the
  * decision bytes as the backtrace reads them back from the buffer, bits[off * 8 + (j - 8 g0)] for a row stored at
  * plane offset off, and the F values at the same offsets in an int16 slab (F1, then F2, ngrp * 8 cells each). */
-template <int GAP>
+template <int GAP, bool PS>
 __global__ void POA_P16_BOUNDS poa_chain_replay_kernel(const __grid_constant__ PoaJobDesc jd, const PoaParamsDev *__restrict__ prm,
                                                        int ring_rows, int ring_cells, const __grid_constant__ P16Consts kc) {
     extern __shared__ __align__(16) uint8_t dyn_smem[];
     const int lane = threadIdx.x;
     const P16Smem sm = p16_smem_init(dyn_smem, prm, ring_rows, lane);
-    p16_run_job<GAP, GLOBAL, true, false, true>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
+    p16_run_job<GAP, GLOBAL, true, false, true, PS>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
 }
 
-template <int GAP>
+template <int GAP, bool PS>
 __global__ void __launch_bounds__(32) poa_fb_dump_kernel(const __grid_constant__ PoaJobDesc jd, const PoaParamsDev *__restrict__ prm, int buf_cells,
                                                          int16_t *fslab, uint8_t *fbits, int32_t *windows, const __grid_constant__ P16Consts kc) {
     extern __shared__ __align__(16) uint8_t dyn_smem[];
@@ -2024,7 +2070,7 @@ __global__ void __launch_bounds__(32) poa_fb_dump_kernel(const __grid_constant__
         const int np = ldb(&jv.rowmeta[i + 1].x) - m0.x;
         uint8_t *ob = fbits + (size_t)off * POA_GROUP;
         for (int j = ri.end; j >= ri.beg; ++n) {
-            const int lo = fb_recompute<GAP, GLOBAL, true>(jv, jd, prm, fx, ri.beg, ri.end, m0.x, np, m0.y & 0xff, j, lane);
+            const int lo = fb_recompute<GAP, GLOBAL, true, PS>(jv, jd, prm, fx, ri.beg, ri.end, m0.x, np, m0.y & 0xff, j, lane);
             for (int c = lo + lane; c <= j; c += 32) ob[c - g0 * 8] = fx.buf[c - lo];
             __syncwarp();
             j = lo - 1;
@@ -2035,44 +2081,47 @@ __global__ void __launch_bounds__(32) poa_fb_dump_kernel(const __grid_constant__
 
 /* largest dynamic shared memory of one CTA (sm_90) */
 #define POA_SMEM_MAX (227 * 1024)
-template <int GAP>
+template <int GAP, bool PS>
 static cudaError_t launch_chain_replay_one(const PoaJobDesc &jd, const PoaParamsDev *prm, int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
     const size_t smem = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
     if (smem > POA_SMEM_MAX) return cudaErrorInvalidValue;
-    cudaError_t e = cudaFuncSetAttribute(poa_chain_replay_kernel<GAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, POA_SMEM_MAX);
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_replay_kernel<GAP, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize, POA_SMEM_MAX);
     if (e != cudaSuccess) return e;
-    poa_chain_replay_kernel<GAP><<<1, 32, smem, st>>>(jd, prm, ring_rows, ring_cells, kc);
+    poa_chain_replay_kernel<GAP, PS><<<1, 32, smem, st>>>(jd, prm, ring_rows, ring_cells, kc);
     return cudaGetLastError();
 }
-/* ring_rows: a power of two >= 2; ring_cells: a positive multiple of 8 (poa_pick_ring gives no less); their ring must fit one CTA */
+/* ring_rows: a power of two >= 2; ring_cells: a positive multiple of 8 (poa_pick_ring gives no less); their ring must fit one CTA.
+ * ps: the job carries -G path scores (the path-score instantiation of the chain's job function) */
 extern "C" cudaError_t poa_launch_chain_replay(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int ring_rows, int ring_cells,
-                                               cudaStream_t st) {
+                                               int ps, cudaStream_t st) {
     if (gap_mode == LG || ring_rows < 2 || (ring_rows & (ring_rows - 1)) || ring_cells < 8 || (ring_cells & 7)) return cudaErrorInvalidValue;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    if (gap_mode == AG) return launch_chain_replay_one<AG>(*jd, prm, ring_rows, ring_cells, kc, st);
-    return launch_chain_replay_one<CG>(*jd, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == AG) return ps ? launch_chain_replay_one<AG, true>(*jd, prm, ring_rows, ring_cells, kc, st) : launch_chain_replay_one<AG, false>(*jd, prm, ring_rows, ring_cells, kc, st);
+    return ps ? launch_chain_replay_one<CG, true>(*jd, prm, ring_rows, ring_cells, kc, st) : launch_chain_replay_one<CG, false>(*jd, prm, ring_rows, ring_cells, kc, st);
 }
 /* the bytes of the chain's backtrace buffer for a ring geometry (fx.buf_cells in p16_run_job) */
 extern "C" int poa_chain_fb_buf_cells(int gap_mode, int ring_rows, int ring_cells) {
     const int rn = gap_mode == LG ? RingPlanes<LG>::N : (gap_mode == AG ? RingPlanes<AG>::N : RingPlanes<CG>::N);
     return rn * ring_cells * 2 * ring_rows;
 }
-template <int GAP>
+template <int GAP, bool PS>
 static cudaError_t launch_fb_dump_one(const PoaJobDesc &jd, const PoaParamsDev *prm, int n_rows, int buf_cells, int16_t *fslab, uint8_t *fbits,
                                       int32_t *windows, const P16Consts &kc, cudaStream_t st) {
     const size_t smem = (size_t)POA_MAX_M * POA_MAX_M * sizeof(int) + 18 * sizeof(uint4) + (size_t)std::max(buf_cells >> 8, 1) * 256;
     if (smem > POA_SMEM_MAX) return cudaErrorInvalidValue;
-    cudaError_t e = cudaFuncSetAttribute(poa_fb_dump_kernel<GAP>, cudaFuncAttributeMaxDynamicSharedMemorySize, POA_SMEM_MAX);
+    cudaError_t e = cudaFuncSetAttribute(poa_fb_dump_kernel<GAP, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize, POA_SMEM_MAX);
     if (e != cudaSuccess) return e;
-    if (n_rows > 2) poa_fb_dump_kernel<GAP><<<n_rows - 2, 32, smem, st>>>(jd, prm, buf_cells, fslab, fbits, windows, kc);
+    if (n_rows > 2) poa_fb_dump_kernel<GAP, PS><<<n_rows - 2, 32, smem, st>>>(jd, prm, buf_cells, fslab, fbits, windows, kc);
     return cudaGetLastError();
 }
 extern "C" cudaError_t poa_launch_fb_dump(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int n_rows, int buf_cells,
-                                          int16_t *fslab, uint8_t *fbits, int32_t *windows, cudaStream_t st) {
+                                          int16_t *fslab, uint8_t *fbits, int32_t *windows, int ps, cudaStream_t st) {
     if (gap_mode == LG) return cudaErrorInvalidValue;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    if (gap_mode == AG) return launch_fb_dump_one<AG>(*jd, prm, n_rows, buf_cells, fslab, fbits, windows, kc, st);
-    return launch_fb_dump_one<CG>(*jd, prm, n_rows, buf_cells, fslab, fbits, windows, kc, st);
+    if (gap_mode == AG) return ps ? launch_fb_dump_one<AG, true>(*jd, prm, n_rows, buf_cells, fslab, fbits, windows, kc, st)
+                                  : launch_fb_dump_one<AG, false>(*jd, prm, n_rows, buf_cells, fslab, fbits, windows, kc, st);
+    return ps ? launch_fb_dump_one<CG, true>(*jd, prm, n_rows, buf_cells, fslab, fbits, windows, kc, st)
+              : launch_fb_dump_one<CG, false>(*jd, prm, n_rows, buf_cells, fslab, fbits, windows, kc, st);
 }
 
 /* ------------------------------------------------------------------ launcher */

@@ -3,10 +3,9 @@
 
 Every read of every group gets deterministic quality-like weights (1..40 per base, seeded per group, as
 tests/cases.py:case_weights draws them).  Runs one batch of a workload per mode (-Q -r 0, -Q -r 2, -G -r 0, -Q -G -r 0 by
-default), once on the device-resident chain engine and once on the launch engine (the ABPOA_GPU_NO_CHAIN flag),
-alternating, and reports per run the wall time, chain_device_ms, chain_groups / chain_fallback_groups and the
-host-to-device / device-to-host bytes.  A mode the chain does not take (-G) runs on the launch engine either way:
-chain_groups stays 0.  It checks that both engines return identical records (consensus, coverage, MSA rows, DP cells,
+default; -G -r 2 on request), once on the device-resident chain engine and once on the launch engine (the
+ABPOA_GPU_NO_CHAIN flag), alternating, and reports per run the wall time, chain_device_ms, chain_groups /
+chain_fallback_groups and the host-to-device / device-to-host bytes.  It checks that both engines return identical records (consensus, coverage, MSA rows, DP cells,
 aligned counts, and every read's score, CIGAR length and CIGAR hash) and prints the card's name and power limit.
 
     python tools/exp_qv.py --workload convex_10k --groups 1000 --reps 1 [--modes Q-r0,Q-r2] [--engines chain]
@@ -30,6 +29,7 @@ MODES = {
     "Q-r2": dict(use_qv=True, out_msa=True, out_cons=True),
     "G-r0": dict(inc_path_score=True, out_msa=False, out_cons=True),
     "QG-r0": dict(use_qv=True, inc_path_score=True, out_msa=False, out_cons=True),
+    "G-r2": dict(inc_path_score=True, out_msa=True, out_cons=True),
 }
 
 
@@ -66,7 +66,7 @@ def main():
     ap.add_argument("--workload", default="convex_10k")
     ap.add_argument("--groups", type=int, default=100)
     ap.add_argument("--reps", type=int, default=1)
-    ap.add_argument("--modes", default=",".join(MODES))
+    ap.add_argument("--modes", default="Q-r0,Q-r2,G-r0,QG-r0")
     ap.add_argument("--engines", choices=["both", "chain", "launch"], default="both")
     args = ap.parse_args()
     wl = synth.WORKLOADS[args.workload]

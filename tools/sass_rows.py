@@ -18,7 +18,7 @@ p16_run_job are cut at its KP(n) phase markers:
 then the backtrace (poa_backtrack and what it calls) and everything else.  The row loop is straight-line per 256-cell
 pass, so at bands up to 256 cells its static count is close to what one row issues.
 
-    python tools/sass_rows.py [--src path/to/poa_kernels.cu] [--gap convex|affine|linear] [--ops]
+    python tools/sass_rows.py [--src path/to/poa_kernels.cu] [--gap convex|affine|linear] [--ops] [--path-score]
 """
 from __future__ import annotations
 
@@ -81,12 +81,13 @@ def regions(src: Path):
     return [(n, a + 1, b + 1) for n, a, b in cuts], [(a + 1, b + 2) for a, b in bt]
 
 
-def disassemble(src: Path, tmp: Path, gap: int):
+def disassemble(src: Path, tmp: Path, gap: int, ps: bool = False):
     cubin = tmp / "k.cubin"
     subprocess.run([NVCC, "-gencode", "arch=compute_90a,code=sm_90a", "-O3", "-lineinfo", "-std=c++17",
                     f"-I{ROOT / 'include'}", f"-I{ROOT / 'abpoa_b200' / 'csrc'}", "-cubin", "-o", str(cubin), str(src)], check=True)
     res = subprocess.run(["/usr/local/cuda/bin/cuobjdump", "-res-usage", str(cubin)], check=True, capture_output=True, text=True).stdout
-    fn = re.search(rf"Function (_Z26poa_chain_dp_worker_kernelILi{gap}E(?:Lb0E)?Ev\w+):", res).group(1)     # without -s
+    tail = "Lb0ELb1E" if ps else "(?:Lb0E)*"                 # without -s; with -G (ps) or without
+    fn = re.search(rf"Function (_Z26poa_chain_dp_worker_kernelILi{gap}E{tail}Ev\w+):", res).group(1)
     m = re.search(re.escape(fn) + r":\s*\n\s*REG:(\d+)", res)
     regs = int(m.group(1)) if m else None
     dis = subprocess.run(["/usr/local/cuda/bin/nvdisasm", "-gi", str(cubin)], check=True, capture_output=True, text=True).stdout
@@ -129,13 +130,14 @@ def main():
     ap.add_argument("--src", type=Path, default=ROOT / "abpoa_b200" / "csrc" / "poa_kernels.cu")
     ap.add_argument("--gap", choices=list(GAPS), default="convex")
     ap.add_argument("--ops", action="store_true", help="also list the most frequent opcodes per region")
+    ap.add_argument("--path-score", action="store_true", help="the path-score (-G) instantiation of the kernel")
     args = ap.parse_args()
     src = args.src.resolve()
     loop_regions, bt_ranges = regions(src)
     with tempfile.TemporaryDirectory() as tmp:
-        text, regs = disassemble(src, Path(tmp), GAPS[args.gap])
+        text, regs = disassemble(src, Path(tmp), GAPS[args.gap], args.path_score)
     counts, ops = count(text, src.name, loop_regions, bt_ranges)
-    print(f"poa_chain_dp_worker_kernel<{args.gap}> from {src.name}: {regs} registers per thread")
+    print(f"poa_chain_dp_worker_kernel<{args.gap}{', -G' if args.path_score else ''}> from {src.name}: {regs} registers per thread")
     print(f"  {'region':<14}{'instructions':>13}")
     row = 0
     for name in LOOP_REGIONS:
