@@ -68,17 +68,18 @@ static_assert(offsetof(PoaChainSync, q_tail) == 128 && offsetof(PoaChainSync, to
 static_assert(POA_GFA_HDR_WORDS == POA_GFA_HDR, "the device's GFA record header is the one poa_gfa_from_record reads");
 
 /* ------------------------------------------------------------------ kernels */
-/* PS: -G runs (ChainCall::ps), whose jobs carry path scores (chain_flatten) */
-template <bool PS>
+/* PS: -G runs (ChainCall::ps), whose jobs carry path scores (chain_flatten); LG: linear-gap runs, whose rows are stored in
+ * whole reference vectors (chain_flatten's plane estimate) */
+template <bool PS, bool LG>
 __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_seed_kernel(PoaChainSlot *slots, const PoaChainParams *cp, int n) {
     if ((int)blockIdx.x >= n) return;
-    chain_seed<PS>(&slots[blockIdx.x], cp);
+    chain_seed<PS, LG>(&slots[blockIdx.x], cp);
 }
 
-template <bool PS>
+template <bool PS, bool LG>
 __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_fuse_kernel(PoaChainSlot *slots, const int32_t *idx, const PoaChainParams *cp, int n, int round) {
     if ((int)blockIdx.x >= n) return;
-    chain_fuse<PS>(&slots[idx[blockIdx.x]], cp, round);
+    chain_fuse<PS, LG>(&slots[idx[blockIdx.x]], cp, round);
 }
 
 /* Free-running chain, fuse side: persistent CTAs draw tickets from PoaChainSync; ticket t is served when tasks[t] holds a group.
@@ -87,7 +88,7 @@ __device__ __forceinline__ int sync_ld(const int32_t *p) { int v; asm volatile("
 __device__ __forceinline__ void sync_st(int32_t *p, int v) { asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ unsigned long long sync_now_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
-template <bool PS>
+template <bool PS, bool LG>
 __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_fuse_worker_kernel(PoaChainSlot *slots, PoaChainSync *sync, const PoaChainParams *cp) {
     __shared__ int task_s;
     for (;;) {
@@ -121,7 +122,7 @@ __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_fuse_worker_kernel(PoaC
         __threadfence();                                       /* acquire: graph arrays / CIGAR of this group may have been written from another SM */
         PoaChainSlot *s = &slots[g];
         const unsigned long long t0 = sync_now_ns();
-        chain_fuse<PS>(s, cp, 0);
+        chain_fuse<PS, LG>(s, cp, 0);
         __syncthreads();
         __threadfence();                                       /* release */
         __syncthreads();
@@ -267,7 +268,6 @@ int poa_chain_eligible(const abpoa_para_t *abpt) {
     if (off && *off == '1') return 0;
     { const char *np = getenv("ABPOA_GPU_NO_P16"); if (np && *np == '1') return 0; }      /* the chain only has the packed int16 kernel */
     if (abpt->align_mode != ABPOA_GLOBAL_MODE || abpt->wb < 0) return 0;
-    if (abpt->gap_mode == ABPOA_LINEAR_GAP) return 0;                      /* banded linear gaps: generic kernel only (lane-exact band edges) */
     /* RC-MSA and GFA run on the chain (per-node read sets, poa_chain_msa_kernel / poa_chain_gfa_kernel), and so does the
      * single-cluster most-frequent-base consensus (it needs n_read per node only; under sub_aln it needs n_span_read,
      * which the device does not keep); use_read_ids is what abpoa_post_set_para sets for them */
@@ -372,6 +372,7 @@ struct ChainCall {
     bool strand;            /* -s: the alignment warp retries weak hits as the reverse complement; read_rc comes back */
     bool qv;                /* -Q and at least one read with weights: every group gets its weight bytes (chain_slot_reads) */
     bool ps;                /* -G: every job blob carries path scores; the kernels' path-score instantiation runs */
+    bool lg;                /* linear gaps: DP rows are stored in whole reference vectors (the seed / fuse kernels' LG instantiation) */
     int sm_count;
 };
 
@@ -395,6 +396,7 @@ ChainCall chain_call(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_worker
     c.mf = abpt->cons_algrm == ABPOA_MF;
     c.strand = abpt->amb_strand != 0;
     c.ps = abpt->inc_path_score != 0;
+    c.lg = abpt->gap_mode == ABPOA_LINEAR_GAP;
     c.qv = false;
     if (abpt->use_qv)
         for (int g : todo)
@@ -454,7 +456,8 @@ std::vector<GroupPlan> plan_groups(const ChainCall &c, const std::vector<int> &t
         const double growth = c.free_run ? 0.032 : 0.045;
         const int band_slack = c.free_run ? 0 : 32;
         const double rows_final = std::min<double>(2.0 + (double)p.bases, (double)p.qmax * (1.0 + growth * (p.n_reads - 1)) + 64);
-        p.pool_units_est = rows_final * (double)((2 * wmax + 1 + band_slack + 7) / 8 + 2) * c.P;
+        const int lg_cells = c.lg ? POA_LG_ROW_CELLS(16) : 0;           /* linear gaps: rows in whole vectors (pn <= 16) */
+        p.pool_units_est = rows_final * (double)((2 * wmax + 1 + band_slack + lg_cells + 7) / 8 + 2) * c.P;
         /* -s: a read that arrives reverse-complemented is first aligned on the wrong strand, and that alignment's band
          * wanders far off the estimate (50 x 10 kbp convex, every third read flipped: slabs of 1.5x the estimate handed
          * 706 of 1000 groups back, slabs of about 6x none).  Fewer groups per wave, each with a larger slab. */
@@ -597,7 +600,7 @@ struct Wave {
             for (int i = 0; i < p.n_reads; ++i) {
                 hoff[i] = acc; acc += in.seq_lens[i];
                 hw[i] = poa_band_halfwidth(c.abpt, in.seq_lens[i]);
-                const int bc = (2 * hw[i] + 1 + 104 + 7) / 8 * 8;
+                const int bc = (2 * hw[i] + 1 + 104 + (c.lg ? POA_LG_ROW_CELLS(16) : 0) + 7) / 8 * 8;
                 if (bc > band_cells) band_cells = bc;
             }
             hoff[p.n_reads] = acc;
@@ -675,8 +678,10 @@ struct Wave {
         h2d = reads_bytes + (uint64_t)nw * sizeof(PoaChainSlot) + sizeof hcp + sizeof hprm + idx.size() * 4 + (uint64_t)nw * 12;
         /* timed region of the device work: inputs are resident when ev_t0 fires */
         CK(cudaEventRecord(ev_t0, s0));
-        if (c.ps) poa_chain_seed_kernel<true><<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw);
-        else poa_chain_seed_kernel<false><<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw);
+        if (c.lg) { if (c.ps) poa_chain_seed_kernel<true, true><<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw);
+                    else poa_chain_seed_kernel<false, true><<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw); }
+        else if (c.ps) poa_chain_seed_kernel<true, false><<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw);
+        else poa_chain_seed_kernel<false, false><<<nw, POA_CHAIN_T, 0, s0>>>(d_slots, d_cp, nw);
         CK(cudaGetLastError());
         CK(cudaEventRecord(ev_up, s0));
         static const size_t smem_budget = [] { const char *e = getenv("ABPOA_GPU_SMEM_KB"); return (size_t)(e && *e ? atoi(e) : 28) * 1024; }();
@@ -722,13 +727,14 @@ struct Wave {
          * with one fuse CTA on every SM (default split of a 5 KB kernel: 64 KB) the alignment grid (split: maximum) never
          * started, and neither kernel ever ends by itself (measured: the fuse workers' watchdog fired, then the alignment
          * grid ran). */
-        CK(cudaFuncSetAttribute(c.ps ? poa_chain_fuse_worker_kernel<true> : poa_chain_fuse_worker_kernel<false>, cudaFuncAttributePreferredSharedMemoryCarveout,
-                                cudaSharedmemCarveoutMaxShared));
+        void (*const fuse_worker)(PoaChainSlot *, PoaChainSync *, const PoaChainParams *) =
+            c.lg ? (c.ps ? poa_chain_fuse_worker_kernel<true, true> : poa_chain_fuse_worker_kernel<false, true>)
+                 : (c.ps ? poa_chain_fuse_worker_kernel<true, false> : poa_chain_fuse_worker_kernel<false, false>);
+        CK(cudaFuncSetAttribute(fuse_worker, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
         static const bool dp_first = [] { const char *e = getenv("ABPOA_GPU_CHAIN_DP_FIRST"); return e && *e == '1'; }();     /* experiment */
         CK(cudaStreamWaitEvent(st_dp, ev_sync, 0));
         if (dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, c.ps, d_prm, ring_rows, ring_cells, st_dp));
-        if (c.ps) poa_chain_fuse_worker_kernel<true><<<n_fuse, POA_CHAIN_T, 0, s0>>>(d_slots, d_sync, d_cp);
-        else poa_chain_fuse_worker_kernel<false><<<n_fuse, POA_CHAIN_T, 0, s0>>>(d_slots, d_sync, d_cp);
+        fuse_worker<<<n_fuse, POA_CHAIN_T, 0, s0>>>(d_slots, d_sync, d_cp);
         CK(cudaGetLastError());
         if (!dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, c.ps, d_prm, ring_rows, ring_cells, st_dp));
         cudaEvent_t ev_dp; CK(cudaEventCreateWithFlags(&ev_dp, cudaEventDisableTiming));
@@ -779,8 +785,10 @@ struct Wave {
                 CK(cudaEventRecord(e0, st));
                 CK(poa_launch_chain_align_p16(c.abpt->gap_mode, gaps, d_slots, d_idx + ro.first, ro.second, r, d_cp, c.strand, c.ps, d_prm, ring_rows, ring_cells, st));
                 CK(cudaEventRecord(e1, st));
-                if (c.ps) poa_chain_fuse_kernel<true><<<ro.second, POA_CHAIN_T, 0, st>>>(d_slots, d_idx + ro.first, d_cp, ro.second, r);
-                else poa_chain_fuse_kernel<false><<<ro.second, POA_CHAIN_T, 0, st>>>(d_slots, d_idx + ro.first, d_cp, ro.second, r);
+                void (*const fuse)(PoaChainSlot *, const int32_t *, const PoaChainParams *, int, int) =
+                    c.lg ? (c.ps ? poa_chain_fuse_kernel<true, true> : poa_chain_fuse_kernel<false, true>)
+                         : (c.ps ? poa_chain_fuse_kernel<true, false> : poa_chain_fuse_kernel<false, false>);
+                fuse<<<ro.second, POA_CHAIN_T, 0, st>>>(d_slots, d_idx + ro.first, d_cp, ro.second, r);
                 CK(cudaGetLastError());
                 CK(cudaEventRecord(e2, st));
                 launches += 2;

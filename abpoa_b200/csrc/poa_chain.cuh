@@ -282,6 +282,10 @@ POA_DEV int chain_ref_pn(const PoaChainParams *cp, int qlen, int n_rows) {
     return max_score <= 32767 - cp->min_mis - cp->oe1 - cp->oe2 ? 16 : 8;
 }
 
+/* linear gaps: cells a DP row stores beyond its band at most -- the band rounded out to whole vectors of pn lanes on both
+ * sides (the reference's banded linear-gap rows, p16_run_job's LGX rows) */
+#define POA_LG_ROW_CELLS(pn) (2 * ((pn) - 1))
+
 POA_DEV size_t chain_al16(size_t x) { return (x + 15) & ~(size_t)15; }
 
 /* -s, reference src/abpoa_align.c:323-325: the forward hit is weak, so the reverse complement is aligned too.  node_n counts
@@ -362,8 +366,10 @@ POA_DEV void chain_set_remain(PoaChainSlot *s, int K, const int32_t *order, int 
 /* Flatten the graph + read `r` into the slot's job blob (layout: PoaJobHeader; the host twin is
  * poa_blob_fill in poa_flat.c).  Also the last line of defence for the order: every predecessor row
  * must be smaller than its row.  PS (-G runs; the host picks the fuse kernels' instantiation, so a run without -G compiles
- * to the bare flatten): the predscore section behind pred, every in-edge's chain_path_score. */
-template <bool PS = false>
+ * to the bare flatten): the predscore section behind pred, every in-edge's chain_path_score.  LG (linear-gap runs, picked
+ * the same way): the DP stores a row in whole reference vectors of pn cells around its band, up to 2 (pn - 1) cells more
+ * (POA_LG_ROW_CELLS). */
+template <bool PS = false, bool LG = false>
 POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int32_t *order, int n, int r, int pool_parity, int generous) {
     const int K = cp->K;
     int32_t *cnt = s->scr[0];
@@ -425,7 +431,7 @@ POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int3
              * that still outgrows the slab comes back as PLANE_OVF and is re-run once with the full rectangle (generous). */
             const int w = s->read_w[r];
             const int drift = qlen > s->rem_row[0] ? qlen - s->rem_row[0] : s->rem_row[0] - qlen;
-            unsigned long long per_row = (unsigned long long)((2 * w + 1 + drift + 64 + 7) / 8 + 2);
+            unsigned long long per_row = (unsigned long long)((2 * w + 1 + drift + 64 + (LG ? POA_LG_ROW_CELLS(h->pn) : 0) + 7) / 8 + 2);
             const unsigned long long full = (unsigned long long)((qlen + 1 + 7) / 8 + 1);
             if (generous || per_row > full) per_row = full;
             const unsigned long long units = per_row * (unsigned long long)cp->P * (unsigned long long)n;
@@ -447,7 +453,7 @@ POA_DEV void chain_flatten(PoaChainSlot *s, const PoaChainParams *cp, const int3
 /* ------------------------------------------------------------------ first read of a group */
 /* a chain SRC -> b0 -> b1 ... -> SINK (reference src/abpoa_graph.c:573-593): the edge into b_i weighs w[i], the edge into
  * SINK w[len - 1]; PS: see chain_flatten */
-template <bool PS = false>
+template <bool PS = false, bool LG = false>
 POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
     const int K = cp->K;
     ChainRead rd = chain_read(s, 0);
@@ -484,7 +490,7 @@ POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
     if (POA_TID0) { s->n_nodes = n; s->cur = 0; s->fused = 1; s->retry = 0; if (s->read_rc) s->read_rc[0] = 0; }   /* read 0 seeds: no strand test */
     POA_CTA_SYNC();
     chain_set_remain(s, K, order, n);
-    if (s->n_reads > 1) chain_flatten<PS>(s, cp, order, n, 1, /*pool_parity=*/1, 0);
+    if (s->n_reads > 1) chain_flatten<PS, LG>(s, cp, order, n, 1, /*pool_parity=*/1, 0);
 }
 
 /* ------------------------------------------------------------------ fuse read r, prepare read r + 1 */
@@ -496,7 +502,7 @@ POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
 /* `round`: the round of the cohort's schedule that just ran (the next alignment kernel is round + 1; its plane pool is
  * the one with that parity).  A group normally fuses read `round`, but one that had to re-run an alignment lags behind.
  * PS: see chain_flatten. */
-template <bool PS = false>
+template <bool PS = false, bool LG = false>
 POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
     const int K = cp->K, A = cp->A;
     const int r = s->fused;                                /* the read whose alignment just finished */
@@ -507,7 +513,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
     if (res->status == POA_ST_PLANE_OVF && !s->retry && s->pool_cursor) {   /* band wider than the slab: same read again, full-rectangle slab */
         POA_CTA_SYNC();
         if (POA_TID0) s->retry = 1;
-        chain_flatten<PS>(s, cp, s->order[s->cur], s->n_nodes, r, round + 1, 1);
+        chain_flatten<PS, LG>(s, cp, s->order[s->cur], s->n_nodes, r, round + 1, 1);
         return;
     }
     if (res->status != POA_ST_OK) {
@@ -707,7 +713,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
 
     /* ---- 9. band centres and the next job ---- */
     chain_set_remain(s, K, order_new, n);
-    if (r + 1 < s->n_reads) chain_flatten<PS>(s, cp, order_new, n, r + 1, round + 1, 0);
+    if (r + 1 < s->n_reads) chain_flatten<PS, LG>(s, cp, order_new, n, r + 1, round + 1, 0);
     else if (POA_TID0) hdr->n_rows = 0;
     POA_CTA_SYNC();
 }

@@ -708,7 +708,11 @@ extern "C" int poa_debug_last_run(abpoa_t *ab, int32_t *out8) {
  * windows recomputed (all rows), windows of the row with the most.
  * A -G alignment (its blob has path scores: off_predscore >= 0) that would have run LEAN but for its path scores replays on
  * the job function's path-score instantiation, as the chain runs -G jobs.
- * Returns -1 unless the last accepted run was the packed LEAN global kernel (or such a -G run) with affine or convex gaps, -2 for a ring that
+ * A banded global linear-gap alignment (the launch engine runs it on the generic kernel's lgx rows) replays on the job
+ * function's linear-gap (LGX) instantiation, as the chain runs linear-gap jobs; its rows are stored in whole reference
+ * vectors, there are no F planes to rebuild (fslab / fbits stay zero) and the replay brings its own query-profile scratch.
+ * Returns -1 unless the last accepted run was the packed LEAN global kernel (or such a -G run) with affine or convex gaps, or
+ * a banded global linear-gap alignment, -2 for a ring that
  * does not fit one CTA or a buffer that does not fit shared memory; else the slab capacity the outputs need (bytes) when
  * `slab` is NULL or `cap` is smaller, else the bytes of the compact slab the replay used.  Nothing of the chain's or the
  * launch engine's own path runs here. */
@@ -720,27 +724,31 @@ extern "C" int poa_chain_fb_buf_cells(int gap_mode, int ring_rows, int ring_cell
 extern "C" int64_t poa_debug_chain_replay(abpoa_t *ab, int ring_rows, int ring_cells, int buf_cells, int32_t *rowinfo, uint32_t *rowoff,
                                           void *slab, void *fslab, uint8_t *fbits, int64_t cap, uint64_t *cigar, int64_t cigar_cap, int64_t *out16) {
     poa_dev_ctx *c = (poa_dev_ctx *)ab->abm->s_mem;
-    if (!c || c->arena || c->last_rows <= 0 || c->last_bits != 15 || !(c->last_lean || c->last_ps)) return -1;
-    if (c->last_gap != ABPOA_AFFINE_GAP && c->last_gap != ABPOA_CONVEX_GAP) return -1;
+    if (!c || c->arena || c->last_rows <= 0) return -1;
+    const bool lin = c->last_gap == ABPOA_LINEAR_GAP;
+    if (!lin && (c->last_bits != 15 || !(c->last_lean || c->last_ps))) return -1;
+    if (!lin && c->last_gap != ABPOA_AFFINE_GAP && c->last_gap != ABPOA_CONVEX_GAP) return -1;
     CK(cudaSetDevice(c->dev));
     PoaJobHeader hd; CK(cudaMemcpy(&hd, c->last_desc.blob, sizeof hd, cudaMemcpyDeviceToHost));
+    PoaParamsDev prm; CK(cudaMemcpy(&prm, c->d_in, sizeof prm, cudaMemcpyDeviceToHost));     /* what the alignment ran with */
+    if (lin && (hd.w < 0 || prm.align_mode != ABPOA_GLOBAL_MODE)) return -1;
     const int n_rows = hd.n_rows, qlen = hd.qlen, gap = c->last_gap, ps = hd.off_predscore >= 0;
-    const int n16 = gap == ABPOA_AFFINE_GAP ? 2 : 3;
+    const int n16 = lin ? 1 : (gap == ABPOA_AFFINE_GAP ? 2 : 3);
     const uint64_t units = (uint64_t)((qlen + 1 + 7) / 8 + 1) * n16 * n_rows;      /* full rectangle: no PLANE_OVF */
     const int64_t need = (int64_t)units * POA_GROUP * 2;
     if (!slab || cap < need) return need;
     if (ring_rows <= 0 || ring_cells <= 0) {
-        const int band_cells = hd.w >= 0 ? (2 * hd.w + 1 + 104 + 7) / 8 * 8 : (qlen + 1 + 7) / 8 * 8 + 8;
+        const int band_cells = hd.w >= 0 ? (2 * hd.w + 1 + 104 + (lin ? 2 * (16 - 1) : 0) + 7) / 8 * 8 : (qlen + 1 + 7) / 8 * 8 + 8;   /* as the chain */
         poa_pick_ring(gap, 16, band_cells, (size_t)28 * 1024, &ring_rows, &ring_cells);
     }
-    PoaParamsDev prm; CK(cudaMemcpy(&prm, c->d_in, sizeof prm, cudaMemcpyDeviceToHost));     /* what the alignment ran with */
     const int gaps[4] = { prm.e1, prm.oe1, prm.e2, prm.oe2 };
     /* fresh outputs: result | rowinfo | rowoff | cigar | btrec | slab | F slab | bytes | windows */
     const size_t o_ri = al256(sizeof(PoaResultDev)), o_ro = o_ri + al256((size_t)n_rows * sizeof(PoaRowInfo));
     const size_t o_cg = o_ro + al256((size_t)n_rows * sizeof(PoaRowOff)), cg_cap = (size_t)qlen + n_rows + 8;
     const size_t o_bt = o_cg + al256(cg_cap * 8), o_sl = o_bt + al256((size_t)n_rows * sizeof(PoaBtRec));
     const size_t o_fs = o_sl + al256((size_t)need), o_fb = o_fs + al256((size_t)need), o_wn = o_fb + al256((size_t)need / 2);
-    const size_t total = o_wn + al256((size_t)n_rows * 4);
+    const size_t o_qp = o_wn + al256((size_t)n_rows * 4);
+    const size_t total = o_qp + al256((size_t)prm.m * ((((size_t)qlen + 1 + 7) & ~(size_t)7) + 8) * 2);
     uint8_t *d = NULL;
     CK(cudaMalloc((void **)&d, total));
     CK(cudaMemset(d, 0, total));
@@ -748,6 +756,7 @@ extern "C" int64_t poa_debug_chain_replay(abpoa_t *ab, int ring_rows, int ring_c
     jd.result = (PoaResultDev *)d; jd.rowinfo = (PoaRowInfo *)(d + o_ri); jd.rowoff = (PoaRowOff *)(d + o_ro);
     jd.cigar = (uint64_t *)(d + o_cg); jd.cigar_cap = (int32_t)cg_cap; jd.btrec = (PoaBtRec *)(d + o_bt);
     jd.planes = d + o_sl; jd.plane_cap_units = units;
+    if (lin) jd.qprof = (int16_t *)(d + o_qp);         /* the generic kernel's launch has no query-profile scratch */
     const cudaError_t le = poa_launch_chain_replay(gap, gaps, &jd, (const PoaParamsDev *)c->d_in, ring_rows, ring_cells, ps, c->st);
     if (le == cudaErrorInvalidValue) { cudaGetLastError(); CK(cudaFree(d)); return -2; }
     CK(le);
@@ -761,7 +770,7 @@ extern "C" int64_t poa_debug_chain_replay(abpoa_t *ab, int ring_rows, int ring_c
     if (buf_cells == 0) buf_cells = poa_chain_fb_buf_cells(gap, ring_rows, ring_cells);
     else if (buf_cells < 0) buf_cells = (max_ngrp + 31) / 32 * 256;
     std::vector<int32_t> win(n_rows, 0);
-    if (r.status == POA_ST_OK) {                        /* every row record is written: the dump reads inside the slab only */
+    if (r.status == POA_ST_OK && !lin) {                /* every row record is written: the dump reads inside the slab only */
         const cudaError_t de = poa_launch_fb_dump(gap, gaps, &jd, (const PoaParamsDev *)c->d_in, n_rows, buf_cells, (int16_t *)(d + o_fs), d + o_fb,
                                                   (int32_t *)(d + o_wn), ps, c->st);
         if (de == cudaErrorInvalidValue) { cudaGetLastError(); CK(cudaFree(d)); return -2; }
@@ -769,7 +778,7 @@ extern "C" int64_t poa_debug_chain_replay(abpoa_t *ab, int ring_rows, int ring_c
         CK(cudaMemcpyAsync(fslab, d + o_fs, (size_t)need, cudaMemcpyDeviceToHost, c->st));
         CK(cudaMemcpyAsync(fbits, d + o_fb, (size_t)need / 2, cudaMemcpyDeviceToHost, c->st));
         CK(cudaMemcpyAsync(win.data(), d + o_wn, (size_t)n_rows * 4, cudaMemcpyDeviceToHost, c->st));
-    }
+    } else if (lin) { memset(fslab, 0, (size_t)need); memset(fbits, 0, (size_t)need / 2); }
     const int n_ops = r.status == POA_ST_OK ? r.n_ops : 0;
     std::vector<uint64_t> ops((size_t)std::max(n_ops, 1));
     if (n_ops > 0) CK(cudaMemcpyAsync(ops.data(), d + o_cg, (size_t)n_ops * 8, cudaMemcpyDeviceToHost, c->st));

@@ -1255,6 +1255,22 @@ __device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaPa
     return lo;
 }
 
+/* LGX rows of p16_run_job (see there).  xs: log2 of the storage granule, one reference vector of pn = 2^xs cells.
+ * First / last stored group of a band [b, e] of a row stored in whole vectors of 2^xs cells */
+__device__ __forceinline__ int p16_xg0(int xs, int b) { return ((b >> xs) << xs) >> 3; }
+__device__ __forceinline__ int p16_xg1(int xs, int e) { return ((((e >> xs) + 1) << xs) - 1) >> 3; }
+/* Predecessor p (band end p_end) feeds the cells j < p_vlim = ((p_end + 1) / pn + 1) * pn only: for group g all of its cells or
+ * none, as p_vlim is a multiple of 8.  For the first predecessor the backtrace shortcut bits (D0) also need j - 1 <= p_end: the
+ * general step takes a diagonal from a cell of the predecessor's band only, never from a leaked cell. */
+__device__ __forceinline__ void p16_lgx_reach(const uint4 *cap_hi, int xs, int g, int p_end, bool first, unsigned &d0, unsigned &d1, unsigned &d2,
+                                              unsigned &d3, uint4 &hp, unsigned (&D0)[4]) {
+    if (first) {
+        const uint4 c = cap_hi[min(max(g * 8 + 7 - (p_end + 1), 0), 8)];
+        D0[0] = __vmins2(d0, c.x); D0[1] = __vmins2(d1, c.y); D0[2] = __vmins2(d2, c.z); D0[3] = __vmins2(d3, c.w);
+    }
+    if (g >= (((((p_end + 1) >> xs) + 1) << xs) >> 3)) { d0 = d1 = d2 = d3 = NEGP2; hp = make_uint4(NEGP2, NEGP2, NEGP2, NEGP2); }
+}
+
 /* One alignment job on one warp: forward DP + backtrace.  Writes *jd.result (every status) but does
  * NOT publish completion -- the caller does (signal_done), after whatever it still has to move. */
 /* LEAN (whole-graph jobs without -G path scores): rows with one or two predecessors that are still in the
@@ -1269,10 +1285,18 @@ __device__ int fb_recompute(const JobView &jv, const PoaJobDesc &jd, const PoaPa
 /* PS (with LEAN; the chain's -G jobs): the job carries path scores.  The straight-line rows add predecessor k's score to its
  * diagonal term and its E planes (linear gaps: to H before - e1), the arithmetic of the general rows, with the scores of the
  * row's first LP predecessors broadcast one row ahead next to their rows.  Without PS a LEAN job carries none. */
-template <int GAP, int MODE, bool LEAN = false, bool TMA = false, bool FB = false, bool PS = false>
+/* LGX (with LEAN; the chain's linear-gap jobs, which are always banded: poa_chain_eligible refuses wb < 0): the rows follow
+ * the reference's vector procedure, as the "lgx" rows of
+ * poa_align_kernel do: a row is stored in whole pn-lane vectors around its band (groups p16_xg0 .. p16_xg1), the cells
+ * end+1 .. xend keep the running value H[end] - k*e1, predecessor p feeds the cells j < p_vlim only (p16_lgx_reach), and
+ * beyond vector V1 = max_p(p.end / pn) + 1 only the even lanes of vector V1 + 1 keep the running value.  In packed form T is
+ * masked on both sides of the band and the stored H by CLO and the group's vector rule (KEEP).  The band (beg / end), the row
+ * maximum and the cell count stay those of the band itself. */
+template <int GAP, int MODE, bool LEAN = false, bool TMA = false, bool FB = false, bool PS = false, bool LGX = false>
 __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParamsDev *__restrict__ prm, const P16Consts &kc, const P16Smem &sm,
                                             int ring_rows, int ring_cells, int lane) {
     static_assert(!(TMA && FB), "the TMA row drain stages the five-plane layout");
+    static_assert(!LGX || (GAP == LG && MODE == GLOBAL && LEAN && !TMA), "lgx rows: linear gaps, global mode, the chain's job function");
     typedef int16_t ST;
     typedef Planes<GAP> PL;
     typedef RowLayout<GAP, FB> RL;
@@ -1311,7 +1335,30 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
     bool stop = false;
 
     /* ---------------- row 0 ---------------- */
-    {
+    if constexpr (LGX) {                                     /* stored up to the end of end0's vector; cells past end0 are -inf */
+        const int xs = pnv == 16 ? 4 : 3;
+        int end0 = qlen;
+        if (banded) end0 = min(qlen, max(0, qlen - jv.remain(0)) + w);
+        const int g1 = p16_xg1(xs, end0), ngrp = g1 + 1;
+        if ((uint64_t)RL::units(ngrp) > jd.plane_cap_units) { if (lane == 0) { res.status = POA_ST_PLANE_OVF; *jd.result = res; } return; }
+        for (int gp = 0; gp <= g1; gp += 32) {
+            const int g = gp + lane;
+            if (g <= g1) {
+                int h[8];
+#pragma unroll
+                for (int c = 0; c < 8; ++c) { const int j = g * 8 + c; h[c] = j > end0 ? NEGP : max(-e1 * j, NEGP); }
+                st8(planes + (size_t)g * POA_GROUP, h);
+                if (g < ring_groups) st8(ring_data + (size_t)g * POA_GROUP, h);
+            }
+        }
+        if (lane == 0) {
+            PoaRowInfo r0; r0.beg = 0; r0.end = end0; r0.left = 0; r0.right = 0;
+            rowinfo[0] = r0; { PoaRowOff z; z.off = 0; z.p0 = -1; rowoff[0] = z; } ring_meta[0] = make_uint4(0u, (unsigned)end0, 1u | (1u << 16), 0u);
+        }
+        cursor = RL::units(ngrp);
+        cells += end0 + 1; max_band = end0 + 1;
+        __syncwarp();
+    } else {
         int end0 = qlen;
         if (banded) end0 = min(qlen, max(0, qlen - jv.remain(0)) + w);
         const int g1 = end0 >> 3, ngrp = g1 + 1;
@@ -1418,10 +1465,12 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
             if (lean_row) {
                 lm[0] = ring_meta[lp[0] & rmask];
                 int wide = (int)(lm[0].y >> 3) - (int)(lm[0].x >> 3) + 1;
+                if constexpr (LGX) wide = p16_xg1(pn_shift, (int)lm[0].y) - p16_xg0(pn_shift, (int)lm[0].x) + 1;
 #pragma unroll
                 for (int k = 1; k < LP; ++k) {
                     lm[k] = k < np ? ring_meta[lp[k] & rmask] : lm[0];
-                    wide = max(wide, (int)(lm[k].y >> 3) - (int)(lm[k].x >> 3) + 1);
+                    if constexpr (LGX) wide = max(wide, p16_xg1(pn_shift, (int)lm[k].y) - p16_xg0(pn_shift, (int)lm[k].x) + 1);
+                    else wide = max(wide, (int)(lm[k].y >> 3) - (int)(lm[k].x >> 3) + 1);
                 }
                 if (wide > ring_groups) lean_row = false;            /* a row wider than its ring slot: only a prefix is cached */
 #ifdef POA_KPROF
@@ -1432,6 +1481,7 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
         /* ---- predecessor k on lane k: band hints + the two broadcast words ---- */
         unsigned wA = 0, wB = 0;                      /* A: pg0 | png<<12 | near<<25 | slot<<26 ; B: plane offset (8-cell units) */
         int l1 = INT32_MAX, r1 = INT32_MIN, b1 = INT32_MAX;
+        int e1x = -1;                                 /* LGX: the predecessor's band end (its reach) */
         if (!lean_row && lane < np) {
             const int prow = mypred;
             const bool near = (i - prow) <= rmask;
@@ -1441,23 +1491,35 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
             l1 = (int)(mi.z & 0xffffu); r1 = (int)(mi.z >> 16); b1 = (int)mi.x;
             const unsigned pg0 = mi.x >> 3, png = (mi.y >> 3) - pg0 + 1;
             wA = pg0 | (png << 12) | ((unsigned)near << 25) | ((unsigned)(prow & rmask) << 26);
+            if constexpr (LGX) {
+                e1x = (int)mi.y;
+                const unsigned xg0 = (unsigned)p16_xg0(pn_shift, (int)mi.x), xng = (unsigned)p16_xg1(pn_shift, (int)mi.y) - xg0 + 1;
+                wA = xg0 | (xng << 12) | ((unsigned)near << 25) | ((unsigned)(prow & rmask) << 26);
+            }
             wB = mi.w;
         }
         int ml = jv.node_n, mr = 0, min_pre_beg = INT32_MAX;
+        int max_pre_end = -1;                         /* LGX */
         if (lean_row) {
 #pragma unroll
             for (int k = 0; k < LP; ++k) {                   /* lm[k >= np] repeats lm[0]: harmless for min / max */
                 ml = min(ml, (int)(lm[k].z & 0xffffu)); mr = max(mr, (int)(lm[k].z >> 16)); min_pre_beg = min(min_pre_beg, (int)lm[k].x);
+                if constexpr (LGX) max_pre_end = max(max_pre_end, (int)lm[k].y);
             }
         } else if (banded) {
             ml = min(ml, __reduce_min_sync(FULL, l1));
             mr = max(mr, __reduce_max_sync(FULL, r1));
             min_pre_beg = __reduce_min_sync(FULL, b1);
+            if constexpr (LGX) max_pre_end = __reduce_max_sync(FULL, e1x);
             for (int kb = 32; kb < np; kb += 32) {          /* more than 32 predecessors: practically never */
                 const int k = kb + lane;
                 int l2 = INT32_MAX, r2 = INT32_MIN, b2 = INT32_MAX;
                 if (k < np) { const PoaRowInfo pi = rowinfo[ldb(jv.pred + pb + k)]; l2 = pi.left + 1; r2 = pi.right + 1; b2 = pi.beg; }
                 ml = min(ml, __reduce_min_sync(FULL, l2)); mr = max(mr, __reduce_max_sync(FULL, r2)); min_pre_beg = min(min_pre_beg, __reduce_min_sync(FULL, b2));
+                if constexpr (LGX) {
+                    const int e2x = k < np ? rowinfo[ldb(jv.pred + pb + k)].end : -1;
+                    max_pre_end = max(max_pre_end, __reduce_max_sync(FULL, e2x));
+                }
             }
         }
         int beg = 0, end = qlen;
@@ -1467,7 +1529,9 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
             end = min(qlen, max(mr, r) + w);
             if (np > 0 && (beg >> pn_shift) < (min_pre_beg >> pn_shift)) beg = min_pre_beg;   /* reference's vector-granular clamp */
         }
-        const int g0 = beg >> 3, g1 = end >> 3, ngrp = g1 - g0 + 1;
+        int g0 = beg >> 3, g1 = end >> 3;
+        if constexpr (LGX) { g0 = p16_xg0(pn_shift, beg); g1 = p16_xg1(pn_shift, end); }
+        const int ngrp = g1 - g0 + 1;
         const uint32_t need = RL::units((uint32_t)ngrp);
         if (need > cap32 - cur32) {
             if (TMA) { if (lane == 0) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); __syncwarp(); }     /* nothing may still read this CTA's smem */
@@ -1516,7 +1580,8 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
                 for (int k = 0; k < LP; ++k) {
                     if (k >= np) break;
                     const uint4 mi = lm[k];
-                    const int pg0 = (int)(mi.x >> 3), png = (int)(mi.y >> 3) - pg0 + 1;
+                    int pg0 = (int)(mi.x >> 3), png = (int)(mi.y >> 3) - pg0 + 1;
+                    if constexpr (LGX) { pg0 = p16_xg0(pn_shift, (int)mi.x); png = p16_xg1(pn_shift, (int)mi.y) - pg0 + 1; }
                     const int rel = g - pg0;
                     const bool inr = active && (unsigned)rel < (unsigned)png;
                     const uint32_t prs = ring_s + (uint32_t)(lp[k] & rmask) * ring_row_bytes;
@@ -1557,9 +1622,10 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
                     if (GAP == LG) {
                         hp.x = __viaddmax_s16x2(hp.x, kc.NE1, NEGP2); hp.y = __viaddmax_s16x2(hp.y, kc.NE1, NEGP2); hp.z = __viaddmax_s16x2(hp.z, kc.NE1, NEGP2); hp.w = __viaddmax_s16x2(hp.w, kc.NE1, NEGP2);
                     }
+                    if constexpr (LGX) p16_lgx_reach(cap_hi, pn_shift, g, (int)mi.y, k == 0, d0, d1, d2, d3, hp, D0);
                     const uint4 x1 = GAP == LG ? hp : ep1;
                     if (k == 0) {
-                        D0[0] = d0; D0[1] = d1; D0[2] = d2; D0[3] = d3;
+                        if constexpr (!LGX) { D0[0] = d0; D0[1] = d1; D0[2] = d2; D0[3] = d3; }
                         M[0] = d0; M[1] = d1; M[2] = d2; M[3] = d3;
                         X1[0] = x1.x; X1[1] = x1.y; X1[2] = x1.z; X1[3] = x1.w;
                         if (GAP == CG) { X2[0] = ep2.x; X2[1] = ep2.y; X2[2] = ep2.z; X2[3] = ep2.w; }
@@ -1572,12 +1638,18 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
             } else
             for (int kb = 0; kb < np; kb += 32) {
                 unsigned cA = wA, cB = wB; int c_ps = myps;
+                int c_end = e1x;
                 if (kb > 0) {
                     const int k = kb + lane; cA = 0; cB = 0; c_ps = 0;
                     if (k < np) {
                         const int prow = ldb(jv.pred + pb + k); const PoaRowInfo pi = rowinfo[prow];
                         const unsigned pg0 = (unsigned)pi.beg >> 3, png = ((unsigned)pi.end >> 3) - pg0 + 1;
                         cA = pg0 | (png << 12); cB = rowoff[prow].off; if (has_ps) c_ps = ldb(jv.predscore + pb + k);
+                        if constexpr (LGX) {
+                            c_end = pi.end;
+                            const unsigned xg0 = (unsigned)p16_xg0(pn_shift, pi.beg), xng = (unsigned)p16_xg1(pn_shift, pi.end) - xg0 + 1;
+                            cA = xg0 | (xng << 12);
+                        }
                     }
                 }
                 const int nk = min(32, np - kb);
@@ -1635,7 +1707,8 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
                             }
                         }
                     }
-                    if (kb == 0 && k == 0) { D0[0] = d0; D0[1] = d1; D0[2] = d2; D0[3] = d3; }
+                    if constexpr (LGX) p16_lgx_reach(cap_hi, pn_shift, g, __shfl_sync(FULL, c_end, k), kb == 0 && k == 0, d0, d1, d2, d3, hp, D0);
+                    else if (kb == 0 && k == 0) { D0[0] = d0; D0[1] = d1; D0[2] = d2; D0[3] = d3; }
                     M[0] = __vmaxs2(M[0], d0); M[1] = __vmaxs2(M[1], d1); M[2] = __vmaxs2(M[2], d2); M[3] = __vmaxs2(M[3], d3);
                     if (GAP == LG) {        /* vertical term H[p][j] - e1 */
                         X1[0] = __vmaxs2(X1[0], __viaddmax_s16x2(hp.x, kc.NE1, NEGP2)); X1[1] = __vmaxs2(X1[1], __viaddmax_s16x2(hp.y, kc.NE1, NEGP2));
@@ -1656,6 +1729,12 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
             const unsigned S[4] = { sv.x, sv.y, sv.z, sv.w };
 
             unsigned H[4], F1[4], F2[4], E1o[4], E2o[4];
+            if constexpr (LGX) {                              /* T inside the band only; H stored from beg to the vector end by KEEP */
+                const int v = (g * 8) >> pn_shift, v1 = (max_pre_end >> pn_shift) + 1;
+                const unsigned keep = v <= v1 ? 0x7fff7fffu : (v == v1 + 1 ? 0x8AD07FFFu : NEGP2);      /* V1 + 1: the even lanes (low halves) */
+                const unsigned HK[4] = { __vmins2(CLO[0], keep), __vmins2(CLO[1], keep), __vmins2(CLO[2], keep), __vmins2(CLO[3], keep) };
+                p16_cells<GAP, MODE>(kc, CAP, HK, S, M, X1, X2, (g - g0) * 8, e1, oe1, e2, oe2, zr2, lane, carry1, carry2, H, F1, F2, E1o, E2o);
+            } else
             p16_cells<GAP, MODE>(kc, CLO, CAP, S, M, X1, X2, (g - g0) * 8, e1, oe1, e2, oe2, zr2, lane, carry1, carry2, H, F1, F2, E1o, E2o);
 
             /* backtrace shortcut record (PoaBtRec): one bit per cell -- is H explained by the first predecessor's diagonal? */
@@ -1708,6 +1787,10 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
             }
 
             KP(3)
+            if constexpr (LGX) {                              /* the row maximum is taken over the band, not the leaked cells */
+#pragma unroll
+                for (int k = 0; k < 4; ++k) H[k] = __vmins2(H[k], CAP[k]);
+            }
             /* row maximum with first / last arg-max; masked cells hold NEGP and never win against a real cell */
             {
                 const int lmax = active ? lane_max8(H) : NEGP;
@@ -1781,7 +1864,8 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
             const int prow = jv.pred[sb + k];
             const PoaRowInfo pi = rowinfo[prow];
             const int endc = qlen > pi.end ? pi.end : qlen;
-            const int pg0 = pi.beg >> 3;
+            int pg0 = pi.beg >> 3;
+            if constexpr (LGX) pg0 = p16_xg0(pn_shift, pi.beg);
             const int v = (endc >= pi.beg) ? (int)planes[(size_t)rowoff[prow].off * POA_GROUP + (endc - pg0 * 8)] : NEG;
             if (v > best_score) { best_score = v; best_i = prow; best_j = endc; }
         }
@@ -1805,7 +1889,8 @@ __device__ __forceinline__ void p16_run_job(const PoaJobDesc &jd, const PoaParam
         FbCtx fx;                                            /* FB: the ring is free now and holds the recomputed decision bytes */
         fx.kc = &kc; fx.cap_lo = cap_lo; fx.cap_hi = cap_hi;
         fx.buf = reinterpret_cast<uint8_t *>(ring_data); fx.buf_cells = (int)ring_row_bytes * ring_rows;
-        poa_backtrack<GAP, ST, MODE, FB, PS>(jv, jd, prm, mat_s, lane, best_i, best_j, *jd.result, 3, jd.btrec, &fx);
+        if constexpr (LGX) poa_backtrack<GAP, ST, MODE, FB, PS>(jv, jd, prm, mat_s, lane, best_i, best_j, *jd.result, pn_shift, jd.btrec, &fx);
+        else poa_backtrack<GAP, ST, MODE, FB, PS>(jv, jd, prm, mat_s, lane, best_i, best_j, *jd.result, 3, jd.btrec, &fx);
         if (lane == 0) jd.result->bt_clk = clock64() - clk1;
     }
 }
@@ -1850,7 +1935,7 @@ __device__ __forceinline__ void chain_align_read(const PoaJobDesc &jd, const Poa
     PoaJobDesc jp = jd;
     bool second = false;
     for (int pass = 0; pass < (STRAND ? 2 : 1); ++pass) {
-        p16_run_job<GAP, GLOBAL, true, false, true, PS>(jp, prm, kc, sm, ring_rows, ring_cells, lane);
+        p16_run_job<GAP, GLOBAL, true, false, true, PS, GAP == LG>(jp, prm, kc, sm, ring_rows, ring_cells, lane);
         __syncwarp();
         if (!STRAND || pass) break;
         const PoaJobHeader *h = reinterpret_cast<const PoaJobHeader *>(jd.blob);
@@ -2046,7 +2131,7 @@ __global__ void POA_P16_BOUNDS poa_chain_replay_kernel(const __grid_constant__ P
     extern __shared__ __align__(16) uint8_t dyn_smem[];
     const int lane = threadIdx.x;
     const P16Smem sm = p16_smem_init(dyn_smem, prm, ring_rows, lane);
-    p16_run_job<GAP, GLOBAL, true, false, true, PS>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
+    p16_run_job<GAP, GLOBAL, true, false, true, PS, GAP == LG>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
 }
 
 template <int GAP, bool PS>
@@ -2094,8 +2179,9 @@ static cudaError_t launch_chain_replay_one(const PoaJobDesc &jd, const PoaParams
  * ps: the job carries -G path scores (the path-score instantiation of the chain's job function) */
 extern "C" cudaError_t poa_launch_chain_replay(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int ring_rows, int ring_cells,
                                                int ps, cudaStream_t st) {
-    if (gap_mode == LG || ring_rows < 2 || (ring_rows & (ring_rows - 1)) || ring_cells < 8 || (ring_cells & 7)) return cudaErrorInvalidValue;
+    if (ring_rows < 2 || (ring_rows & (ring_rows - 1)) || ring_cells < 8 || (ring_cells & 7)) return cudaErrorInvalidValue;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
+    if (gap_mode == LG) return ps ? launch_chain_replay_one<LG, true>(*jd, prm, ring_rows, ring_cells, kc, st) : launch_chain_replay_one<LG, false>(*jd, prm, ring_rows, ring_cells, kc, st);
     if (gap_mode == AG) return ps ? launch_chain_replay_one<AG, true>(*jd, prm, ring_rows, ring_cells, kc, st) : launch_chain_replay_one<AG, false>(*jd, prm, ring_rows, ring_cells, kc, st);
     return ps ? launch_chain_replay_one<CG, true>(*jd, prm, ring_rows, ring_cells, kc, st) : launch_chain_replay_one<CG, false>(*jd, prm, ring_rows, ring_cells, kc, st);
 }
