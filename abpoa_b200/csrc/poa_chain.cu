@@ -26,7 +26,9 @@
  * that fit the arena (split_waves) and runs each wave (Wave).  A group's device region is laid out by chain_slot_layout
  * (poa_chain.cuh) for the planner and the carve alike.
  *
- * Scope of the chain: global alignment, banded (wb >= 0), packed-int16 admissible scores, heaviest-bundling or
+ * Scope of the chain: global alignment, or extend alignment (-m 2, with or without z-drop -z; affine or convex gaps: the
+ * alignment kernels' EXTEND instantiation, rows in the reference's Kahn order, chain_kahn_order), banded (wb >= 0),
+ * packed-int16 admissible scores, heaviest-bundling or
  * most-frequent-base consensus (single cluster, no sub_aln), row-column MSA and GFA (one read set per node, not per
  * edge), base weights (-Q: a weight byte per read base, 0..255; a group with any other weight takes the other engine),
  * ambiguous strand (-s: the alignment warp retries a weak hit as the reverse complement, chain_align_read in
@@ -56,11 +58,11 @@
     poa_die("libabpoa_b200/chain", "%s failed at %s:%d: %s", #call, __FILE__, __LINE__, cudaGetErrorString(e_)); } while (0)
 
 extern "C" cudaError_t poa_launch_chain_dp_worker(int gap_mode, const int *gaps, PoaChainSlot *slots, PoaChainSync *sync, int n_groups,
-                                                  const PoaChainParams *cp, int strand, int ps, const PoaParamsDev *prm, int ring_rows, int ring_cells,
-                                                  cudaStream_t st);
+                                                  const PoaChainParams *cp, int strand, int ps, int ext, const PoaParamsDev *prm, int ring_rows,
+                                                  int ring_cells, cudaStream_t st);
 extern "C" cudaError_t poa_launch_chain_align_p16(int gap_mode, const int *gaps, const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round,
-                                                  const PoaChainParams *cp, int strand, int ps, const PoaParamsDev *prm, int ring_rows, int ring_cells,
-                                                  cudaStream_t st);
+                                                  const PoaChainParams *cp, int strand, int ps, int ext, const PoaParamsDev *prm, int ring_rows,
+                                                  int ring_cells, cudaStream_t st);
 extern "C" void poa_pick_ring(int gap_mode, int bits, int band_cells, size_t smem_budget, int *ring_rows, int *ring_cells);
 
 static_assert(offsetof(PoaChainSync, q_tail) == 128 && offsetof(PoaChainSync, total) == 256 && offsetof(PoaChainSync, abort) == 384,
@@ -69,17 +71,18 @@ static_assert(POA_GFA_HDR_WORDS == POA_GFA_HDR, "the device's GFA record header 
 
 /* ------------------------------------------------------------------ kernels */
 /* PS: -G runs (ChainCall::ps), whose jobs carry path scores (chain_flatten); LG: linear-gap runs, whose rows are stored in
- * whole reference vectors (chain_flatten's plane estimate) */
+ * whole reference vectors (chain_flatten's plane estimate); KO: extend runs, whose rows follow the reference's Kahn order
+ * (chain_fuse) */
 template <bool PS, bool LG>
 __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_seed_kernel(PoaChainSlot *slots, const PoaChainParams *cp, int n) {
     if ((int)blockIdx.x >= n) return;
     chain_seed<PS, LG>(&slots[blockIdx.x], cp);
 }
 
-template <bool PS, bool LG>
+template <bool PS, bool LG, bool KO = false>
 __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_fuse_kernel(PoaChainSlot *slots, const int32_t *idx, const PoaChainParams *cp, int n, int round) {
     if ((int)blockIdx.x >= n) return;
-    chain_fuse<PS, LG>(&slots[idx[blockIdx.x]], cp, round);
+    chain_fuse<PS, LG, KO>(&slots[idx[blockIdx.x]], cp, round);
 }
 
 /* Free-running chain, fuse side: persistent CTAs draw tickets from PoaChainSync; ticket t is served when tasks[t] holds a group.
@@ -88,7 +91,7 @@ __device__ __forceinline__ int sync_ld(const int32_t *p) { int v; asm volatile("
 __device__ __forceinline__ void sync_st(int32_t *p, int v) { asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ unsigned long long sync_now_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
-template <bool PS, bool LG>
+template <bool PS, bool LG, bool KO = false>
 __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_fuse_worker_kernel(PoaChainSlot *slots, PoaChainSync *sync, const PoaChainParams *cp) {
     __shared__ int task_s;
     for (;;) {
@@ -122,7 +125,7 @@ __global__ void __launch_bounds__(POA_CHAIN_T) poa_chain_fuse_worker_kernel(PoaC
         __threadfence();                                       /* acquire: graph arrays / CIGAR of this group may have been written from another SM */
         PoaChainSlot *s = &slots[g];
         const unsigned long long t0 = sync_now_ns();
-        chain_fuse<PS, LG>(s, cp, 0);
+        chain_fuse<PS, LG, KO>(s, cp, 0);
         __syncthreads();
         __threadfence();                                       /* release */
         __syncthreads();
@@ -267,14 +270,17 @@ int poa_chain_eligible(const abpoa_para_t *abpt) {
     const char *off = getenv("ABPOA_GPU_NO_CHAIN");
     if (off && *off == '1') return 0;
     { const char *np = getenv("ABPOA_GPU_NO_P16"); if (np && *np == '1') return 0; }      /* the chain only has the packed int16 kernel */
-    if (abpt->align_mode != ABPOA_GLOBAL_MODE || abpt->wb < 0) return 0;
+    /* extend mode (-m 2, with or without z-drop): banded, affine or convex gaps (the linear-gap rows are global-only) */
+    const int ext = abpt->align_mode == ABPOA_EXTEND_MODE;
+    if ((abpt->align_mode != ABPOA_GLOBAL_MODE && !ext) || abpt->wb < 0) return 0;
+    if (ext && abpt->gap_mode == ABPOA_LINEAR_GAP) return 0;
     /* RC-MSA and GFA run on the chain (per-node read sets, poa_chain_msa_kernel / poa_chain_gfa_kernel), and so does the
      * single-cluster most-frequent-base consensus (it needs n_read per node only; under sub_aln it needs n_span_read,
      * which the device does not keep); use_read_ids is what abpoa_post_set_para sets for them */
     const int mf = abpt->cons_algrm == ABPOA_MF && abpt->use_read_ids && !abpt->sub_aln;
     if (abpt->cons_algrm != ABPOA_HB && !mf) return 0;
     if ((abpt->use_read_ids && !abpt->out_msa && !abpt->out_gfa && !mf) || abpt->max_n_cons > 1) return 0;
-    if (abpt->zdrop > 0 || abpt->rev_cigar || !abpt->ret_cigar) return 0;
+    if ((abpt->zdrop > 0 && !ext) || abpt->rev_cigar || !abpt->ret_cigar) return 0;
     if (abpt->put_gap_on_right || abpt->put_gap_at_end) return 0;         /* handled by the kernels, but keep the chain on the common configuration */
     if (abpt->m > POA_MAX_M) return 0;
     if (!(abpt->disable_seeding && abpt->progressive_poa == 0)) return 0;
@@ -373,6 +379,7 @@ struct ChainCall {
     bool qv;                /* -Q and at least one read with weights: every group gets its weight bytes (chain_slot_reads) */
     bool ps;                /* -G: every job blob carries path scores; the kernels' path-score instantiation runs */
     bool lg;                /* linear gaps: DP rows are stored in whole reference vectors (the seed / fuse kernels' LG instantiation) */
+    bool ext;               /* extend mode: the alignment kernels' EXTEND and the fuse kernels' Kahn-order (KO) instantiations */
     int sm_count;
 };
 
@@ -397,6 +404,7 @@ ChainCall chain_call(int dev, poa_arena *arena, abpoa_para_t *abpt, int n_worker
     c.strand = abpt->amb_strand != 0;
     c.ps = abpt->inc_path_score != 0;
     c.lg = abpt->gap_mode == ABPOA_LINEAR_GAP;
+    c.ext = abpt->align_mode == ABPOA_EXTEND_MODE;
     c.qv = false;
     if (abpt->use_qv)
         for (int g : todo)
@@ -428,11 +436,16 @@ std::vector<GroupPlan> plan_groups(const ChainCall &c, const std::vector<int> &t
         /* -G: a node weighs at most n_reads x the largest weight; past POA_PS_MAX_NODE_W the device's log is not known to round
          * as the host's does */
         if (c.ps && (int64_t)in.n_seq * (c.qv ? 255 : 1) > POA_PS_MAX_NODE_W) ok = false;
+        /* extend: chain_kahn_order keeps an in-degree (<= K) in a byte */
+        if (c.ext && c.K > 254) ok = false;
         if (!ok || p.qmax > (1 << 24)) { fallback.push_back(g); continue; }
         /* node capacity: 10 % growth per read, and for large groups at most 4 % plus a fixed slack (5 % error, 50 x 10 kbp:
          * 3.0 % measured, 33.8k nodes reserved for 25k used) -- a group that outgrows it goes to the launch engine */
-        const int64_t grow = std::min<int64_t>((int64_t)((double)p.qmax * (1.0 + 0.10 * (p.n_reads - 1))) + 256,
-                                               (int64_t)((double)p.qmax * (1.0 + 0.04 * (p.n_reads - 1))) + 4096);
+        int64_t grow = std::min<int64_t>((int64_t)((double)p.qmax * (1.0 + 0.10 * (p.n_reads - 1))) + 256,
+                                         (int64_t)((double)p.qmax * (1.0 + 0.04 * (p.n_reads - 1))) + 4096);
+        /* extend runs: a read whose best cell lies before its end (z-drop, high error) threads the rest of it as new nodes:
+         * room for every base up to 16k nodes (25 % error groups of a few hundred bases outgrew 10 % per read) */
+        if (c.ext) grow = std::max<int64_t>(grow, 16384);
         p.n_cap = (int)std::min<int64_t>(2 + p.bases, grow);
         /* what the wave carve will take for the group, at its 256-byte granularity */
         PoaChainSlot probe;
@@ -728,15 +741,16 @@ struct Wave {
          * started, and neither kernel ever ends by itself (measured: the fuse workers' watchdog fired, then the alignment
          * grid ran). */
         void (*const fuse_worker)(PoaChainSlot *, PoaChainSync *, const PoaChainParams *) =
-            c.lg ? (c.ps ? poa_chain_fuse_worker_kernel<true, true> : poa_chain_fuse_worker_kernel<false, true>)
-                 : (c.ps ? poa_chain_fuse_worker_kernel<true, false> : poa_chain_fuse_worker_kernel<false, false>);
+            c.ext ? (c.ps ? poa_chain_fuse_worker_kernel<true, false, true> : poa_chain_fuse_worker_kernel<false, false, true>)
+            : c.lg ? (c.ps ? poa_chain_fuse_worker_kernel<true, true> : poa_chain_fuse_worker_kernel<false, true>)
+                   : (c.ps ? poa_chain_fuse_worker_kernel<true, false> : poa_chain_fuse_worker_kernel<false, false>);
         CK(cudaFuncSetAttribute(fuse_worker, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
         static const bool dp_first = [] { const char *e = getenv("ABPOA_GPU_CHAIN_DP_FIRST"); return e && *e == '1'; }();     /* experiment */
         CK(cudaStreamWaitEvent(st_dp, ev_sync, 0));
-        if (dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, c.ps, d_prm, ring_rows, ring_cells, st_dp));
+        if (dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, c.ps, c.ext, d_prm, ring_rows, ring_cells, st_dp));
         fuse_worker<<<n_fuse, POA_CHAIN_T, 0, s0>>>(d_slots, d_sync, d_cp);
         CK(cudaGetLastError());
-        if (!dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, c.ps, d_prm, ring_rows, ring_cells, st_dp));
+        if (!dp_first) CK(poa_launch_chain_dp_worker(c.abpt->gap_mode, gaps, d_slots, d_sync, nw, d_cp, c.strand, c.ps, c.ext, d_prm, ring_rows, ring_cells, st_dp));
         cudaEvent_t ev_dp; CK(cudaEventCreateWithFlags(&ev_dp, cudaEventDisableTiming));
         CK(cudaEventRecord(ev_dp, st_dp));
         CK(cudaStreamWaitEvent(s0, ev_dp, 0));
@@ -783,11 +797,12 @@ struct Wave {
                 cudaEvent_t e0, e1, e2; CK(cudaEventCreate(&e0)); CK(cudaEventCreate(&e1)); CK(cudaEventCreate(&e2));
                 coh[k].marks.push_back(e0); coh[k].marks.push_back(e1); coh[k].marks.push_back(e2);
                 CK(cudaEventRecord(e0, st));
-                CK(poa_launch_chain_align_p16(c.abpt->gap_mode, gaps, d_slots, d_idx + ro.first, ro.second, r, d_cp, c.strand, c.ps, d_prm, ring_rows, ring_cells, st));
+                CK(poa_launch_chain_align_p16(c.abpt->gap_mode, gaps, d_slots, d_idx + ro.first, ro.second, r, d_cp, c.strand, c.ps, c.ext, d_prm, ring_rows, ring_cells, st));
                 CK(cudaEventRecord(e1, st));
                 void (*const fuse)(PoaChainSlot *, const int32_t *, const PoaChainParams *, int, int) =
-                    c.lg ? (c.ps ? poa_chain_fuse_kernel<true, true> : poa_chain_fuse_kernel<false, true>)
-                         : (c.ps ? poa_chain_fuse_kernel<true, false> : poa_chain_fuse_kernel<false, false>);
+                    c.ext ? (c.ps ? poa_chain_fuse_kernel<true, false, true> : poa_chain_fuse_kernel<false, false, true>)
+                    : c.lg ? (c.ps ? poa_chain_fuse_kernel<true, true> : poa_chain_fuse_kernel<false, true>)
+                           : (c.ps ? poa_chain_fuse_kernel<true, false> : poa_chain_fuse_kernel<false, false>);
                 fuse<<<ro.second, POA_CHAIN_T, 0, st>>>(d_slots, d_idx + ro.first, d_cp, ro.second, r);
                 CK(cudaGetLastError());
                 CK(cudaEventRecord(e2, st));

@@ -10,8 +10,9 @@
  *   edge order (exchange pass)     reference src/abpoa_graph.c:192-219
  *   max_remain                     reference src/abpoa_graph.c:268-309
  *   pre_index / query set-up       reference src/abpoa_align_simd.c:463-560
- * The topological order is the SPLICED order of poa_graph.c (global mode: the DP result does not
- * depend on which topological order the rows follow), not the reference's Kahn order.
+ * The topological order is the SPLICED order of poa_graph.c in global mode (the DP result does not
+ * depend on which topological order the rows follow), and the reference's FIFO Kahn order in extend
+ * mode (chain_kahn_order: the best cell and the z-drop stop are the first row in row order that meets them).
  *
  * How it is written: one CTA per read group; the body is a sequence of data-parallel PHASES
  * (POA_PAR_FOR loops separated by CTA barriers) plus block scans.  A read's path visits every
@@ -51,7 +52,7 @@
 #define POA_CF_NODE_CAP   0x01          /* node capacity of the slot exhausted            */
 #define POA_CF_EDGE_CAP   0x02          /* a node needs more than K in- or out-edges       */
 #define POA_CF_ALN_CAP    0x04          /* an aligned set needs more than A members        */
-#define POA_CF_ORDER      0x08          /* the spliced order would not be topological      */
+#define POA_CF_ORDER      0x08          /* the spliced / Kahn order would not be topological */
 #define POA_CF_BLOB_CAP   0x10          /* flattened job does not fit the slot's blob      */
 #define POA_CF_DP_STATUS  0x20          /* the DP kernel reported RANGE / PLANE_OVF / ...  */
 #define POA_CF_CIGAR      0x40          /* graph-CIGAR inconsistent with the read          */
@@ -363,6 +364,74 @@ POA_DEV void chain_set_remain(PoaChainSlot *s, int K, const int32_t *order, int 
     }
 }
 
+/* Extend mode: the reference's row order (host twin abpoa_BFS_set_node_index in poa_graph.c, reference
+ * src/abpoa_graph.c:221-266) into order[] / node_row[]: FIFO Kahn from SRC, stopping when SINK is dequeued; out-edges in
+ * list order; a node in an aligned set becomes ready only when every member's in-degree is 0, and the set is then
+ * enqueued as the trigger node followed by its aligned list.  The host walks the out-lists BEFORE the read's weight
+ * changes are re-ordered (order_edges_by_weight runs after the walk), so chain_fuse<.., KO> leaves its out-lists in
+ * append / bump order and re-orders them behind this walk.  The queue is order[] itself.
+ * The CTA precomputes, per node, its in-degree counter (a byte in scr[2]; CHAIN_KAHN_LINK for a "chain link": one in-edge
+ * and no aligned set, ready as soon as its predecessor is dequeued) and, when the node's only out-edge enters a chain
+ * link, that successor (scr[3]); the walk itself is serial on thread 0 (a POA graph is about as deep as it is long) and
+ * costs one dependent load per node on a run of chain links.  Needs K <= 254 (plan_groups).  Needs the whole CTA. */
+#define CHAIN_KAHN_LINK 0xff
+POA_DEV void chain_kahn_order(PoaChainSlot *s, const PoaChainParams *cp, int32_t *order, int n) {
+    const int K = cp->K, A = cp->A;
+    uint8_t *deg = reinterpret_cast<uint8_t *>(s->scr[2]);
+    int32_t *nx = s->scr[3];
+    POA_PAR_FOR(v, n) {
+        const int ni = s->in_cnt[v];
+        deg[v] = (ni == 1 && s->aln_cnt[v] == 0) ? (uint8_t)CHAIN_KAHN_LINK : (uint8_t)ni;
+    }
+    POA_CTA_SYNC();
+    POA_PAR_FOR(u, n) {
+        int x = -1;
+        if (s->out_cnt[u] == 1) { const int v = s->out_id[(size_t)u * K]; if (deg[v] == CHAIN_KAHN_LINK) x = v; }
+        nx[u] = x;
+    }
+    POA_CTA_SYNC();
+    if (POA_TID0) {
+        int head = 0, tail = 1, last = 0, done = 0;
+        order[0] = 0;
+        while (head < tail) {
+            const int cur = head + 1 == tail ? last : order[head];      /* a queue of one: the node just pushed, from a register */
+            s->node_row[cur] = head++;
+            if (cur == 1) { done = head == n; break; }
+            const int x = nx[cur];
+            if (x >= 0) {                                                /* a run of chain links */
+                if (tail >= n) break;
+                order[tail++] = last = x;
+                continue;
+            }
+            const int ne = s->out_cnt[cur];
+            const int32_t *oid = s->out_id + (size_t)cur * K;
+            int full = 0;
+            for (int e = 0; e < ne && !full; ++e) {
+                const int v = oid[e];
+                int d = deg[v];
+                if (d != CHAIN_KAHN_LINK) {
+                    deg[v] = (uint8_t)--d;
+                    if (d != 0) continue;
+                    const int na = s->aln_cnt[v];
+                    const int32_t *al = s->aln_id + (size_t)v * A;
+                    int ready = 1;
+                    for (int a = 0; a < na; ++a) if (deg[al[a]] != 0) { ready = 0; break; }
+                    if (!ready) continue;
+                    if (tail + 1 + na > n) { full = 1; break; }
+                    order[tail++] = last = v;
+                    for (int a = 0; a < na; ++a) order[tail++] = last = al[a];
+                } else {
+                    if (tail >= n) { full = 1; break; }
+                    order[tail++] = last = v;
+                }
+            }
+            if (full) break;
+        }
+        if (!done) POA_ATOMIC_OR(&s->failed, POA_CF_ORDER);     /* not a DAG, or SINK came before a node: not a POA graph */
+    }
+    POA_CTA_SYNC();
+}
+
 /* Flatten the graph + read `r` into the slot's job blob (layout: PoaJobHeader; the host twin is
  * poa_blob_fill in poa_flat.c).  Also the last line of defence for the order: every predecessor row
  * must be smaller than its row.  PS (-G runs; the host picks the fuse kernels' instantiation, so a run without -G compiles
@@ -501,8 +570,10 @@ POA_DEV void chain_seed(PoaChainSlot *s, const PoaChainParams *cp) {
 
 /* `round`: the round of the cohort's schedule that just ran (the next alignment kernel is round + 1; its plane pool is
  * the one with that parity).  A group normally fuses read `round`, but one that had to re-run an alignment lags behind.
- * PS: see chain_flatten. */
-template <bool PS = false, bool LG = false>
+ * PS: see chain_flatten.  KO (extend runs; the host picks the fuse kernels' instantiation): the new order is the
+ * reference's Kahn order (chain_kahn_order) instead of the splice of steps 4 and 8, and the out-lists are re-ordered by
+ * weight behind it.  The seed's chain order is already the Kahn order of a path. */
+template <bool PS = false, bool LG = false, bool KO = false>
 POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
     const int K = cp->K, A = cp->A;
     const int r = s->fused;                                /* the read whose alignment just finished */
@@ -579,7 +650,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
                 const int na = s->aln_cnt[v]; const int32_t *al = s->aln_id + (size_t)v * A;
                 for (int a = 0; a < na; ++a) if (s->base[al[a]] == b) { target = al[a]; break; }
                 if (target >= 0) kind = CK_OLD;
-                else { kind = CK_NEWM; anchor = chain_group_last_row(s, A, order, old_n, v); target = v; }   /* target: the column's node for now */
+                else { kind = CK_NEWM; anchor = KO ? -1 : chain_group_last_row(s, A, order, old_n, v); target = v; }   /* target: the column's node for now */
             }
         }
         tgt[qi] = target; isnew[qi] = kind != CK_OLD;
@@ -601,6 +672,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
      *         mismatch node      -> behind the aligned group of its column
      *         inserted after old -> behind the aligned group of the previous path node
      *         inserted after new -> inherits the previous new node's anchor                      ---- */
+    if (!KO) {
     POA_PAR_FOR(qi, qlen) {
         const int kind = kind_anchor[qi] >> 28;
         int anchor = -1;
@@ -623,6 +695,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
             }
         }
         POA_CTA_SYNC();
+    }
     }
 
     /* ---- 5. create the new nodes; final targets ---- */
@@ -655,7 +728,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
                 if (iid[i] == from) { iw[i] += w; found = 1; if (i > 0 && iw[i - 1] < iw[i]) chain_exchange_order(iid, iw, nin); break; }
             if (found)
                 for (int i = 0; i < nout; ++i)
-                    if (oid[i] == to) { ow[i] += w; if (i > 0 && ow[i - 1] < ow[i]) chain_exchange_order(oid, ow, nout); break; }
+                    if (oid[i] == to) { ow[i] += w; if (!KO && i > 0 && ow[i - 1] < ow[i]) chain_exchange_order(oid, ow, nout); break; }
         }
         if (!found) {
             if (nin >= K || nout >= K) POA_ATOMIC_OR(&s->failed, POA_CF_EDGE_CAP);
@@ -663,7 +736,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
                 iid[nin] = from; iw[nin] = w; s->in_cnt[to] = ++nin;
                 if (nin > 1 && iw[nin - 2] < w) chain_exchange_order(iid, iw, nin);
                 oid[nout] = to; ow[nout] = w; s->out_cnt[from] = ++nout;
-                if (nout > 1 && ow[nout - 2] < w) chain_exchange_order(oid, ow, nout);
+                if (!KO && nout > 1 && ow[nout - 2] < w) chain_exchange_order(oid, ow, nout);
             }
         }
         s->n_read[from] += 1;
@@ -693,7 +766,14 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
     if (s->failed) { if (POA_TID0) hdr->n_rows = 0; POA_CTA_SYNC(); return; }
 
     /* ---- 8. splice: old row i moves up by the number of new nodes anchored in front of it; the k-th new node
-     *         (anchors non-decreasing along the path) lands at anchor_k + 1 + k ---- */
+     *         (anchors non-decreasing along the path) lands at anchor_k + 1 + k.
+     *         KO: the Kahn walk instead, then the out-lists by weight (the exchange pass leaves a sorted list alone) ---- */
+    if (KO) {
+        chain_kahn_order(s, cp, order_new, n);
+        POA_PAR_FOR(v, n) { const int no = s->out_cnt[v]; if (no > 1) chain_exchange_order(s->out_id + (size_t)v * K, s->out_w + (size_t)v * K, no); }
+        POA_CTA_SYNC();
+        if (s->failed) { if (POA_TID0) hdr->n_rows = 0; POA_CTA_SYNC(); return; }
+    } else {
     POA_PAR_FOR(k, n_new) { if (k > 0 && new_anchor[k] < new_anchor[k - 1]) POA_ATOMIC_OR(&s->failed, POA_CF_ORDER); }
     POA_CTA_SYNC();
     if (s->failed) { if (POA_TID0) hdr->n_rows = 0; POA_CTA_SYNC(); return; }
@@ -708,6 +788,7 @@ POA_DEV void chain_fuse(PoaChainSlot *s, const PoaChainParams *cp, int round) {
         order_new[nr] = v; s->node_row[v] = nr;
     }
     POA_CTA_SYNC();
+    }
     if (POA_TID0) { s->n_nodes = n; s->cur ^= 1; s->fused = r + 1; s->retry = 0; }
     POA_CTA_SYNC();
 

@@ -711,13 +711,16 @@ extern "C" int poa_debug_last_run(abpoa_t *ab, int32_t *out8) {
  * A banded global linear-gap alignment (the launch engine runs it on the generic kernel's lgx rows) replays on the job
  * function's linear-gap (LGX) instantiation, as the chain runs linear-gap jobs; its rows are stored in whole reference
  * vectors, there are no F planes to rebuild (fslab / fbits stay zero) and the replay brings its own query-profile scratch.
- * Returns -1 unless the last accepted run was the packed LEAN global kernel (or such a -G run) with affine or convex gaps, or
- * a banded global linear-gap alignment, -2 for a ring that
+ * A banded whole-graph extend alignment (-m 2; the launch engine runs it on the packed kernel's general rows) replays on the
+ * job function's EXTEND instantiation, as the chain runs extend jobs; the F-plane dump rebuilds its rows as global ones
+ * (the recompute differs by mode only in local mode).
+ * Returns -1 unless the last accepted run was the packed LEAN global kernel (or such a -G run, or such an extend run) with
+ * affine or convex gaps, or a banded global linear-gap alignment, -2 for a ring that
  * does not fit one CTA or a buffer that does not fit shared memory; else the slab capacity the outputs need (bytes) when
  * `slab` is NULL or `cap` is smaller, else the bytes of the compact slab the replay used.  Nothing of the chain's or the
  * launch engine's own path runs here. */
 extern "C" cudaError_t poa_launch_chain_replay(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int ring_rows, int ring_cells,
-                                               int ps, cudaStream_t st);
+                                               int ps, int ext, cudaStream_t st);
 extern "C" cudaError_t poa_launch_fb_dump(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int n_rows, int buf_cells,
                                           int16_t *fslab, uint8_t *fbits, int32_t *windows, int ps, cudaStream_t st);
 extern "C" int poa_chain_fb_buf_cells(int gap_mode, int ring_rows, int ring_cells);
@@ -726,11 +729,13 @@ extern "C" int64_t poa_debug_chain_replay(abpoa_t *ab, int ring_rows, int ring_c
     poa_dev_ctx *c = (poa_dev_ctx *)ab->abm->s_mem;
     if (!c || c->arena || c->last_rows <= 0) return -1;
     const bool lin = c->last_gap == ABPOA_LINEAR_GAP;
-    if (!lin && (c->last_bits != 15 || !(c->last_lean || c->last_ps))) return -1;
-    if (!lin && c->last_gap != ABPOA_AFFINE_GAP && c->last_gap != ABPOA_CONVEX_GAP) return -1;
     CK(cudaSetDevice(c->dev));
     PoaJobHeader hd; CK(cudaMemcpy(&hd, c->last_desc.blob, sizeof hd, cudaMemcpyDeviceToHost));
     PoaParamsDev prm; CK(cudaMemcpy(&prm, c->d_in, sizeof prm, cudaMemcpyDeviceToHost));     /* what the alignment ran with */
+    /* a banded whole-graph extend alignment of the packed kernel replays on the chain's EXTEND instantiation */
+    const bool ext = !lin && c->last_bits == 15 && prm.align_mode == ABPOA_EXTEND_MODE && hd.w >= 0 && hd.off_live < 0;
+    if (!lin && (c->last_bits != 15 || !(c->last_lean || c->last_ps || ext))) return -1;
+    if (!lin && c->last_gap != ABPOA_AFFINE_GAP && c->last_gap != ABPOA_CONVEX_GAP) return -1;
     if (lin && (hd.w < 0 || prm.align_mode != ABPOA_GLOBAL_MODE)) return -1;
     const int n_rows = hd.n_rows, qlen = hd.qlen, gap = c->last_gap, ps = hd.off_predscore >= 0;
     const int n16 = lin ? 1 : (gap == ABPOA_AFFINE_GAP ? 2 : 3);
@@ -757,7 +762,7 @@ extern "C" int64_t poa_debug_chain_replay(abpoa_t *ab, int ring_rows, int ring_c
     jd.cigar = (uint64_t *)(d + o_cg); jd.cigar_cap = (int32_t)cg_cap; jd.btrec = (PoaBtRec *)(d + o_bt);
     jd.planes = d + o_sl; jd.plane_cap_units = units;
     if (lin) jd.qprof = (int16_t *)(d + o_qp);         /* the generic kernel's launch has no query-profile scratch */
-    const cudaError_t le = poa_launch_chain_replay(gap, gaps, &jd, (const PoaParamsDev *)c->d_in, ring_rows, ring_cells, ps, c->st);
+    const cudaError_t le = poa_launch_chain_replay(gap, gaps, &jd, (const PoaParamsDev *)c->d_in, ring_rows, ring_cells, ps, ext, c->st);
     if (le == cudaErrorInvalidValue) { cudaGetLastError(); CK(cudaFree(d)); return -2; }
     CK(le);
     PoaResultDev r; CK(cudaMemcpyAsync(&r, d, sizeof r, cudaMemcpyDeviceToHost, c->st));

@@ -1927,15 +1927,18 @@ static inline size_t ring_smem_bytes(int gap, int bits, int ring_rows, int ring_
  * strictly more; its CIGAR words and result are then copied over the primary ones, so the fuse reads one place either
  * way.  The primary result carries the DP cells and cycles of both passes and the first status that is not OK (a failed
  * pair is re-run or handed back like a failed alignment); read_rc[r] records the strand (bit 0) and whether the retry
- * ran (bit 1).  PS (-G; the host picks the instantiation): the job blob carries path scores (p16_run_job). */
-template <int GAP, bool STRAND, bool PS>
+ * ran (bit 1).  PS (-G; the host picks the instantiation): the job blob carries path scores (p16_run_job).  EXT (extend
+ * runs, -m 2; the host picks the instantiation): the EXTEND rows -- the same straight-line LEAN rows and compact layout,
+ * then the best cell of the first row that holds the maximum and the z-drop stop (prm->zdrop); the job's rows follow the
+ * reference's Kahn order (chain_fuse's KO). */
+template <int GAP, bool STRAND, bool PS, bool EXT = false>
 __device__ __forceinline__ void chain_align_read(const PoaJobDesc &jd, const PoaChainSlot *sl, const PoaChainParams *__restrict__ cp,
                                                  const PoaParamsDev *__restrict__ prm, const P16Consts &kc, const P16Smem &sm, int ring_rows, int ring_cells,
                                                  int lane) {
     PoaJobDesc jp = jd;
     bool second = false;
     for (int pass = 0; pass < (STRAND ? 2 : 1); ++pass) {
-        p16_run_job<GAP, GLOBAL, true, false, true, PS, GAP == LG>(jp, prm, kc, sm, ring_rows, ring_cells, lane);
+        p16_run_job<GAP, EXT ? EXTEND : GLOBAL, true, false, true, PS, GAP == LG && !EXT>(jp, prm, kc, sm, ring_rows, ring_cells, lane);
         __syncwarp();
         if (!STRAND || pass) break;
         const PoaJobHeader *h = reinterpret_cast<const PoaJobHeader *>(jd.blob);
@@ -1970,7 +1973,7 @@ __device__ __forceinline__ void chain_align_read(const PoaJobDesc &jd, const Poa
  * The same job function, fed from device-resident slots (poa_chain.cuh): the job blob of a slot is written
  * by the fuse kernel of the previous round, nothing comes from the host.  Block 0 also zeroes the plane-pool
  * cursor the coming fuse kernel will fill (see PoaChainSlot). */
-template <int GAP, bool STRAND, bool PS>
+template <int GAP, bool STRAND, bool PS, bool EXT = false>
 __global__ void POA_P16_BOUNDS poa_chain_align_kernel_p16(const PoaChainSlot *__restrict__ slots, const int32_t *__restrict__ idx,
                                                            const PoaChainParams *__restrict__ cp, const PoaParamsDev *__restrict__ prm, int n_jobs,
                                                            int round, int ring_rows, int ring_cells, const __grid_constant__ P16Consts kc) {
@@ -1984,7 +1987,7 @@ __global__ void POA_P16_BOUNDS poa_chain_align_kernel_p16(const PoaChainSlot *__
     const int n_rows = reinterpret_cast<const PoaJobHeader *>(jd.blob)->n_rows;
     if (sl->failed || sl->fused >= sl->n_reads || n_rows < 3) { if (lane == 0) jd.result->status = POA_ST_SKIP; return; }
     const P16Smem sm = p16_smem_init(dyn_smem, prm, ring_rows, lane);
-    chain_align_read<GAP, STRAND, PS>(jd, sl, cp, prm, kc, sm, ring_rows, ring_cells, lane);
+    chain_align_read<GAP, STRAND, PS, EXT>(jd, sl, cp, prm, kc, sm, ring_rows, ring_cells, lane);
 }
 
 /* Free-running chain (PoaChainSync in poa_chain.cuh): one resident warp per group runs the group's alignments back to
@@ -1994,7 +1997,7 @@ __device__ __forceinline__ int chain_ld_relaxed(const int32_t *p) { int v; asm v
 __device__ __forceinline__ void chain_st_relaxed(int32_t *p, int v) { asm volatile("st.relaxed.gpu.global.s32 [%0], %1;" :: "l"(p), "r"(v) : "memory"); }
 __device__ __forceinline__ unsigned long long chain_now_ns() { unsigned long long t; asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t)); return t; }
 
-template <int GAP, bool STRAND, bool PS>
+template <int GAP, bool STRAND, bool PS, bool EXT = false>
 __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, PoaChainSync *sync, const PoaChainParams *__restrict__ cp,
                                                           const PoaParamsDev *__restrict__ prm, int n_groups, int ring_rows, int ring_cells, int dbg,
                                                           const __grid_constant__ P16Consts kc) {
@@ -2034,7 +2037,7 @@ __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, P
         const PoaJobDesc jd = sl->jd;
         const int n_rows = reinterpret_cast<const PoaJobHeader *>(jd.blob)->n_rows;
         if (sl->failed || sl->fused >= sl->n_reads || n_rows < 3) break;
-        chain_align_read<GAP, STRAND, PS>(jd, sl, cp, prm, kc, sm, ring_rows, ring_cells, lane);
+        chain_align_read<GAP, STRAND, PS, EXT>(jd, sl, cp, prm, kc, sm, ring_rows, ring_cells, lane);
         __syncwarp();
         if (!(dbg & 1)) __threadfence();                       /* release side: CIGAR + result are out before the task is */
         if (lane == 0) {
@@ -2053,7 +2056,7 @@ __global__ void POA_P16_BOUNDS poa_chain_dp_worker_kernel(PoaChainSlot *slots, P
     }
 }
 
-template <int GAP, bool STRAND, bool PS>
+template <int GAP, bool STRAND, bool PS, bool EXT>
 static cudaError_t launch_chain_worker_one(PoaChainSlot *slots, PoaChainSync *sync, int n_groups, const PoaChainParams *cp, const PoaParamsDev *prm,
                                            int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
     /* at least 23 KB: at most 9 of these CTAs fit one SM, which leaves registers (9 x 160 x 32 of 64 K) and shared memory for a
@@ -2062,60 +2065,75 @@ static cudaError_t launch_chain_worker_one(PoaChainSlot *slots, PoaChainSync *sy
     static const int dbg = [] { const char *e = getenv("ABPOA_GPU_CHAIN_DBG"); return e && *e ? atoi(e) : 0; }();
     const size_t smem0 = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
     const size_t smem = (dbg & 2) ? smem0 : std::max<size_t>(smem0, (size_t)23 * 1024);
-    cudaError_t e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, STRAND, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, STRAND, PS, EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return e;
     /* the same L1/shared split as the fuse workers ask for (poa_chain.cu): CTAs of both kernels share SMs for the whole run */
     { const char *cv = getenv("ABPOA_GPU_CHAIN_CARVEOUT");
-      e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, STRAND, PS>, cudaFuncAttributePreferredSharedMemoryCarveout, cv && *cv ? atoi(cv) : (int)cudaSharedmemCarveoutMaxShared);
+      e = cudaFuncSetAttribute(poa_chain_dp_worker_kernel<GAP, STRAND, PS, EXT>, cudaFuncAttributePreferredSharedMemoryCarveout, cv && *cv ? atoi(cv) : (int)cudaSharedmemCarveoutMaxShared);
       if (e != cudaSuccess) return e; }
-    poa_chain_dp_worker_kernel<GAP, STRAND, PS><<<n_groups, 32, smem, st>>>(slots, sync, cp, prm, n_groups, ring_rows, ring_cells, dbg, kc);
+    poa_chain_dp_worker_kernel<GAP, STRAND, PS, EXT><<<n_groups, 32, smem, st>>>(slots, sync, cp, prm, n_groups, ring_rows, ring_cells, dbg, kc);
     return cudaGetLastError();
 }
-template <bool STRAND, bool PS>
+template <bool STRAND, bool PS, bool EXT>
 static cudaError_t launch_chain_worker_gap(int gap_mode, PoaChainSlot *slots, PoaChainSync *sync, int n_groups, const PoaChainParams *cp,
                                            const PoaParamsDev *prm, int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
-    if (gap_mode == LG) return launch_chain_worker_one<LG, STRAND, PS>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
-    if (gap_mode == AG) return launch_chain_worker_one<AG, STRAND, PS>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
-    return launch_chain_worker_one<CG, STRAND, PS>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    if constexpr (EXT) { if (gap_mode == LG) return cudaErrorInvalidValue; }          /* linear-gap extend: not on the chain */
+    else if (gap_mode == LG) return launch_chain_worker_one<LG, STRAND, PS, false>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == AG) return launch_chain_worker_one<AG, STRAND, PS, EXT>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    return launch_chain_worker_one<CG, STRAND, PS, EXT>(slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
 }
-/* strand / ps: the host's PoaChainParams::amb_strand (-s) and whether the run has -G path scores, which pick the kernel instantiation */
+template <bool EXT>
+static cudaError_t launch_chain_worker_ext(int gap_mode, PoaChainSlot *slots, PoaChainSync *sync, int n_groups, const PoaChainParams *cp, int strand,
+                                           int ps, const PoaParamsDev *prm, int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
+    if (strand) return ps ? launch_chain_worker_gap<true, true, EXT>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st)
+                          : launch_chain_worker_gap<true, false, EXT>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    return ps ? launch_chain_worker_gap<false, true, EXT>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st)
+              : launch_chain_worker_gap<false, false, EXT>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+}
+/* strand / ps / ext: the host's PoaChainParams::amb_strand (-s), whether the run has -G path scores and whether it is an extend
+ * run (-m 2), which pick the kernel instantiation */
 extern "C" cudaError_t poa_launch_chain_dp_worker(int gap_mode, const int *gaps, PoaChainSlot *slots, PoaChainSync *sync, int n_groups,
-                                                  const PoaChainParams *cp, int strand, int ps, const PoaParamsDev *prm, int ring_rows, int ring_cells,
-                                                  cudaStream_t st) {
+                                                  const PoaChainParams *cp, int strand, int ps, int ext, const PoaParamsDev *prm, int ring_rows,
+                                                  int ring_cells, cudaStream_t st) {
     if (n_groups <= 0) return cudaSuccess;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    if (strand) return ps ? launch_chain_worker_gap<true, true>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st)
-                          : launch_chain_worker_gap<true, false>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
-    return ps ? launch_chain_worker_gap<false, true>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st)
-              : launch_chain_worker_gap<false, false>(gap_mode, slots, sync, n_groups, cp, prm, ring_rows, ring_cells, kc, st);
+    return ext ? launch_chain_worker_ext<true>(gap_mode, slots, sync, n_groups, cp, strand, ps, prm, ring_rows, ring_cells, kc, st)
+               : launch_chain_worker_ext<false>(gap_mode, slots, sync, n_groups, cp, strand, ps, prm, ring_rows, ring_cells, kc, st);
 }
 
-template <int GAP, bool STRAND, bool PS>
+template <int GAP, bool STRAND, bool PS, bool EXT>
 static cudaError_t launch_chain_one(const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round, const PoaChainParams *cp, const PoaParamsDev *prm,
                                     int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
     const size_t smem = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
-    cudaError_t e = cudaFuncSetAttribute(poa_chain_align_kernel_p16<GAP, STRAND, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_align_kernel_p16<GAP, STRAND, PS, EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)(227 * 1024));
     if (e != cudaSuccess) return e;
-    poa_chain_align_kernel_p16<GAP, STRAND, PS><<<n_jobs, 32, smem, st>>>(slots, idx, cp, prm, n_jobs, round, ring_rows, ring_cells, kc);
+    poa_chain_align_kernel_p16<GAP, STRAND, PS, EXT><<<n_jobs, 32, smem, st>>>(slots, idx, cp, prm, n_jobs, round, ring_rows, ring_cells, kc);
     return cudaGetLastError();
 }
-template <bool STRAND, bool PS>
+template <bool STRAND, bool PS, bool EXT>
 static cudaError_t launch_chain_gap(int gap_mode, const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round, const PoaChainParams *cp,
                                     const PoaParamsDev *prm, int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
-    if (gap_mode == LG) return launch_chain_one<LG, STRAND, PS>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
-    if (gap_mode == AG) return launch_chain_one<AG, STRAND, PS>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
-    return launch_chain_one<CG, STRAND, PS>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    if constexpr (EXT) { if (gap_mode == LG) return cudaErrorInvalidValue; }          /* linear-gap extend: not on the chain */
+    else if (gap_mode == LG) return launch_chain_one<LG, STRAND, PS, false>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    if (gap_mode == AG) return launch_chain_one<AG, STRAND, PS, EXT>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    return launch_chain_one<CG, STRAND, PS, EXT>(slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+}
+template <bool EXT>
+static cudaError_t launch_chain_ext(int gap_mode, const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round, const PoaChainParams *cp,
+                                    int strand, int ps, const PoaParamsDev *prm, int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
+    if (strand) return ps ? launch_chain_gap<true, true, EXT>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st)
+                          : launch_chain_gap<true, false, EXT>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    return ps ? launch_chain_gap<false, true, EXT>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st)
+              : launch_chain_gap<false, false, EXT>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
 }
 /* gaps[4] = { e1, oe1, e2, oe2 } (host copy of what prm holds on the device) */
 extern "C" cudaError_t poa_launch_chain_align_p16(int gap_mode, const int *gaps, const PoaChainSlot *slots, const int32_t *idx, int n_jobs, int round,
-                                                  const PoaChainParams *cp, int strand, int ps, const PoaParamsDev *prm, int ring_rows, int ring_cells,
-                                                  cudaStream_t st) {
+                                                  const PoaChainParams *cp, int strand, int ps, int ext, const PoaParamsDev *prm, int ring_rows,
+                                                  int ring_cells, cudaStream_t st) {
     if (n_jobs <= 0) return cudaSuccess;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
-    if (strand) return ps ? launch_chain_gap<true, true>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st)
-                          : launch_chain_gap<true, false>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
-    return ps ? launch_chain_gap<false, true>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st)
-              : launch_chain_gap<false, false>(gap_mode, slots, idx, n_jobs, round, cp, prm, ring_rows, ring_cells, kc, st);
+    return ext ? launch_chain_ext<true>(gap_mode, slots, idx, n_jobs, round, cp, strand, ps, prm, ring_rows, ring_cells, kc, st)
+               : launch_chain_ext<false>(gap_mode, slots, idx, n_jobs, round, cp, strand, ps, prm, ring_rows, ring_cells, kc, st);
 }
 
 /* ------------------------------------------------------------------ debug: the chain's job function on one job
@@ -2125,13 +2143,13 @@ extern "C" cudaError_t poa_launch_chain_align_p16(int gap_mode, const int *gaps,
  * the row's last cell first, then at the cell left of the previous window, down to the band's first cell.  It keeps the
  * decision bytes as the backtrace reads them back from the buffer, bits[off * 8 + (j - 8 g0)] for a row stored at
  * plane offset off, and the F values at the same offsets in an int16 slab (F1, then F2, ngrp * 8 cells each). */
-template <int GAP, bool PS>
+template <int GAP, bool PS, bool EXT = false>
 __global__ void POA_P16_BOUNDS poa_chain_replay_kernel(const __grid_constant__ PoaJobDesc jd, const PoaParamsDev *__restrict__ prm,
                                                        int ring_rows, int ring_cells, const __grid_constant__ P16Consts kc) {
     extern __shared__ __align__(16) uint8_t dyn_smem[];
     const int lane = threadIdx.x;
     const P16Smem sm = p16_smem_init(dyn_smem, prm, ring_rows, lane);
-    p16_run_job<GAP, GLOBAL, true, false, true, PS, GAP == LG>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
+    p16_run_job<GAP, EXT ? EXTEND : GLOBAL, true, false, true, PS, GAP == LG && !EXT>(jd, prm, kc, sm, ring_rows, ring_cells, lane);
 }
 
 template <int GAP, bool PS>
@@ -2166,21 +2184,27 @@ __global__ void __launch_bounds__(32) poa_fb_dump_kernel(const __grid_constant__
 
 /* largest dynamic shared memory of one CTA (sm_90) */
 #define POA_SMEM_MAX (227 * 1024)
-template <int GAP, bool PS>
+template <int GAP, bool PS, bool EXT = false>
 static cudaError_t launch_chain_replay_one(const PoaJobDesc &jd, const PoaParamsDev *prm, int ring_rows, int ring_cells, const P16Consts &kc, cudaStream_t st) {
     const size_t smem = ring_smem_bytes(GAP, 16, ring_rows, ring_cells) + 18 * sizeof(uint4);
     if (smem > POA_SMEM_MAX) return cudaErrorInvalidValue;
-    cudaError_t e = cudaFuncSetAttribute(poa_chain_replay_kernel<GAP, PS>, cudaFuncAttributeMaxDynamicSharedMemorySize, POA_SMEM_MAX);
+    cudaError_t e = cudaFuncSetAttribute(poa_chain_replay_kernel<GAP, PS, EXT>, cudaFuncAttributeMaxDynamicSharedMemorySize, POA_SMEM_MAX);
     if (e != cudaSuccess) return e;
-    poa_chain_replay_kernel<GAP, PS><<<1, 32, smem, st>>>(jd, prm, ring_rows, ring_cells, kc);
+    poa_chain_replay_kernel<GAP, PS, EXT><<<1, 32, smem, st>>>(jd, prm, ring_rows, ring_cells, kc);
     return cudaGetLastError();
 }
 /* ring_rows: a power of two >= 2; ring_cells: a positive multiple of 8 (poa_pick_ring gives no less); their ring must fit one CTA.
- * ps: the job carries -G path scores (the path-score instantiation of the chain's job function) */
+ * ps: the job carries -G path scores (the path-score instantiation of the chain's job function); ext: an extend job (the
+ * chain's EXTEND instantiation; affine or convex gaps) */
 extern "C" cudaError_t poa_launch_chain_replay(int gap_mode, const int *gaps, const PoaJobDesc *jd, const PoaParamsDev *prm, int ring_rows, int ring_cells,
-                                               int ps, cudaStream_t st) {
+                                               int ps, int ext, cudaStream_t st) {
     if (ring_rows < 2 || (ring_rows & (ring_rows - 1)) || ring_cells < 8 || (ring_cells & 7)) return cudaErrorInvalidValue;
     const P16Consts kc = make_p16_consts(gaps[0], gaps[1], gaps[2], gaps[3]);
+    if (ext) {
+        if (gap_mode == LG) return cudaErrorInvalidValue;
+        if (gap_mode == AG) return ps ? launch_chain_replay_one<AG, true, true>(*jd, prm, ring_rows, ring_cells, kc, st) : launch_chain_replay_one<AG, false, true>(*jd, prm, ring_rows, ring_cells, kc, st);
+        return ps ? launch_chain_replay_one<CG, true, true>(*jd, prm, ring_rows, ring_cells, kc, st) : launch_chain_replay_one<CG, false, true>(*jd, prm, ring_rows, ring_cells, kc, st);
+    }
     if (gap_mode == LG) return ps ? launch_chain_replay_one<LG, true>(*jd, prm, ring_rows, ring_cells, kc, st) : launch_chain_replay_one<LG, false>(*jd, prm, ring_rows, ring_cells, kc, st);
     if (gap_mode == AG) return ps ? launch_chain_replay_one<AG, true>(*jd, prm, ring_rows, ring_cells, kc, st) : launch_chain_replay_one<AG, false>(*jd, prm, ring_rows, ring_cells, kc, st);
     return ps ? launch_chain_replay_one<CG, true>(*jd, prm, ring_rows, ring_cells, kc, st) : launch_chain_replay_one<CG, false>(*jd, prm, ring_rows, ring_cells, kc, st);

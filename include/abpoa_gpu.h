@@ -14,11 +14,12 @@
  *
  * Two engines sit behind abpoa_gpu_msa_batch (DESIGN.md section 5).  The device-resident CHAIN engine keeps
  * the graph of every group in HBM and runs align -> fuse -> re-order -> flatten entirely on the GPU (global,
+ * or extend -m 2 with or without z-drop on affine / convex gaps with the reference's Kahn row order built on the device;
  * banded, convex / affine / linear gaps, heaviest-bundling or most-frequent-base consensus, RC-MSA or GFA output, ambiguous
  * strand -s, quality weights -Q of 0..255, path scores -G): two persistent kernels per batch -- one resident warp per group
  * running its alignments back to back, one fuse CTA per SM serving a task queue -- so every group advances at
  * its own pace; reads go up once, consensus bytes, MSA rows and GFA records come back once.  Everything else --
- * local / extend mode, -d > 1, -a 1 with sub_aln, a weight outside 0..255, -G groups that could weigh more than 2^20 at a
+ * local mode, linear-gap extend, -d > 1, -a 1 with sub_aln, a weight outside 0..255, -G groups that could weigh more than 2^20 at a
  * node, groups that outgrow their device slot -- runs on the
  * LAUNCH engine: worker threads flatten and fuse on the host and launch one kernel grid per round, each
  * worker keeping ABPOA_GPU_PIPE_DEPTH sub-chunks in flight.  Same results either way.
